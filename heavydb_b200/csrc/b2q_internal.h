@@ -161,7 +161,6 @@ struct DevProgram {
   int8_t eager_key;      /* load the key column for every row, overlapped with the filter columns */
   int8_t eager_args;     /* load aggregate arguments for every row instead of only the passing ones */
   int8_t col_width[B2Q_MAX_COLS];    /* byte width of launch column c */
-  int8_t col_prefetch[B2Q_MAX_COLS]; /* column is read for (nearly) every row: worth a bulk L2 prefetch ahead of the scan */
   int8_t fused;          /* shared-memory-table fast path: the program is {COUNT(*)} and/or {one integer SUM without a
                             NULL test}: both updates of a row happen under ONE predicate region */
   int8_t fused_cnt;      /* accumulator index of the COUNT(*), or -1 */

@@ -37,7 +37,7 @@ int32_t make_query(const B2QExecUnit* u, const B2QTableInfo* t, const B2QExecuti
 int scan_rows_per_chunk(int block);
 void scan_config(const B2QQuery& q, int* block, int* ctas_per_sm);
 cudaError_t launch_scan(const B2QQuery& q, const DevLaunch& launch, const int8_t* smem_image, int block, int ctas_per_sm,
-                        int prefetch_distance, cudaStream_t st);
+                        cudaStream_t st);
 cudaError_t launch_init(const B2QQuery& q, int64_t* const* accs, int64_t* keys, int8_t* smem_image, cudaStream_t st);
 cudaError_t launch_join_build(const int8_t* keys, int width, int64_t n_rows, int64_t min_key, int64_t entry_count, int nullable,
                               int64_t null_val, int32_t* buff, int32_t* error, const int8_t* packed_vals, int packed_width,
@@ -74,24 +74,6 @@ static int32_t set_err(int32_t code, const std::string& m) {
                      std::string(#call) + ": " + cudaGetErrorString(e__));                                     \
     }                                                                                                          \
   } while (0)
-
-/* TMA bulk L2 prefetch distance (chunks ahead per CTA); needs 16-byte aligned column pointers.  B2Q_PREFETCH_DISTANCE
- * overrides the default for experiments (0 disables). */
-static int prefetch_distance_for(const B2QQuery& q, const std::vector<const int8_t*>& cols) {
-  /* D=1 helps the shared-memory-table kernels, a long distance thrashes L2, and the L2-resident-table kernels want L2
-   * for the table, not for the stream */
-  static int env = []() {
-    const char* e = getenv("B2Q_PREFETCH_DISTANCE");
-    return e ? atoi(e) : -1;
-  }();
-  const bool smem_kernel = q.plan.kernel == B2Q_KERNEL_PERFECT_SMEM || q.plan.kernel == B2Q_KERNEL_NON_GROUPED;
-  /* the join kernels are bound by the L2 gathers of the probe: a prefetched stream only competes with them */
-  const bool join_kernel = q.prog.join.fk_col >= 0;
-  const int dist = env >= 0 ? env : (smem_kernel && !join_kernel ? 1 : 0);
-  if (dist <= 0) return 0;
-  for (const int8_t* p : cols) if (reinterpret_cast<uintptr_t>(p) & 15) return 0;
-  return dist;
-}
 
 static bool have_device() {
   int n = 0;
@@ -437,7 +419,7 @@ static int32_t scan_device_fragments(B2QPartial& p, int nf, const std::vector<co
     const int32_t rc = radix_launch(p, L, st);
     if (rc != B2Q_OK) return rc;
   } else {
-    CU(launch_scan(q, L, p.smem_image, block, ctas, prefetch_distance_for(q, cols), st));
+    CU(launch_scan(q, L, p.smem_image, block, ctas, st));
     p.launches += 1;
   }
   if (time_it) { CU(cudaEventRecord(p.ev[3], st)); p.scan_timed = true; }
@@ -606,7 +588,7 @@ static int32_t scan_host_table(B2QPartial& p, const B2QTableInfo& tbl, const B2Q
       rc = radix_launch(p, L, st);
       if (rc != B2Q_OK) break;
     } else {
-      cudaError_t e = launch_scan(q, L, p.smem_image, block, ctas, 0 /* slices arrive straight from PCIe */, st);
+      cudaError_t e = launch_scan(q, L, p.smem_image, block, ctas, st);
       if (e != cudaSuccess) { rc = set_err(B2Q_ERR_CUDA, std::string("scan launch: ") + cudaGetErrorString(e)); break; }
       p.launches += 1;
     }

@@ -291,14 +291,12 @@ void scan_config(const B2QQuery& q, int* block, int* ctas_per_sm) {
 }
 
 cudaError_t launch_scan(const B2QQuery& q, const DevLaunch& launch, const int8_t* smem_image, int block, int ctas_per_sm,
-                        int prefetch_distance, cudaStream_t st) {
+                        cudaStream_t st) {
   ScanArgs a;
   a.prog = q.prog;
   a.launch = launch;
   a.smem = q.smem;
   a.smem_image = smem_image;
-  a.prefetch_distance = prefetch_distance;
-  a.pad_ = 0;
   a.ndv_bitmap_bytes = q.plan.query_desc_type == B2Q_Estimator ? q.plan.buffer_size : 0;
   ScanConfig c;
   c.block = block;

@@ -1360,7 +1360,6 @@ class Planner {
         d.translate_null = !kt.notnull && phys_int_null(c) != kt.int_null();
         d.null_val = phys_int_null(c);
         d.null_logical = kt.int_null();
-        g.col_prefetch[d.col] = 1;
       }
       g.key.col = -1;
       g.key.entry_count = 1;
@@ -1377,10 +1376,7 @@ class Planner {
       EL.touched_acc = -1;
       EL.touch_via_acc = -1;
       EL.keyless_marker = -1;
-      for (int t = 0; t < g.filter.n_terms; ++t) { g.col_prefetch[g.filter.terms[t].col] = 1; if (g.filter.terms[t].col2 >= 0) g.col_prefetch[g.filter.terms[t].col2] = 1; }
-      if (join_) g.col_prefetch[g.join.fk_col] = 1;
       g.join.packed_col = -1;
-      for (int c = 0; c < g.n_cols; ++c) if (g.col_inner[c]) g.col_prefetch[c] = 0;
       return;
     }
 
@@ -1532,12 +1528,6 @@ class Planner {
       }
     }
     if (grouped_ && !p.keyless_hash && !L.baseline) L.touched_acc = find_or_add_acc(q, make_acc(q, ACC_TOUCH, nullptr));
-    /* columns worth prefetching: filter columns always; key / arguments when they are loaded eagerly */
-    for (int t = 0; t < g.filter.n_terms; ++t) { g.col_prefetch[g.filter.terms[t].col] = 1; if (g.filter.terms[t].col2 >= 0) g.col_prefetch[g.filter.terms[t].col2] = 1; }
-    if (grouped_ && g.eager_key) { if (g.n_keys > 1) { for (int i = 0; i < g.n_keys; ++i) g.col_prefetch[g.keys[i].col] = 1; } else g.col_prefetch[g.key.col] = 1; }
-    if (g.eager_args)
-      for (int a = 0; a < g.n_accs; ++a) if (g.accs[a].col >= 0) g.col_prefetch[g.accs[a].col] = 1;
-    if (join_) g.col_prefetch[g.join.fk_col] = 1;
     g.join.packed_col = -1;
     g.join.probe_cg = []() { const char* e = getenv("B2Q_JOIN_CG"); return e && atoi(e) != 0; }() ? 1 : 0;
     if (join_) { /* the first 1/2/4-byte inner column the program reads rides in the join table itself */
@@ -1566,7 +1556,6 @@ class Planner {
         g.join.slot16_min = vr.imin;
       }
     }
-    for (int c = 0; c < g.n_cols; ++c) if (g.col_inner[c]) g.col_prefetch[c] = 0; /* gathered by join index, not streamed */
     /* fused fast path of the shared-memory-table kernel (the reference's JIT specialises per query; this is the
      * static-kernel equivalent for the most common shape: GROUP BY k with COUNT(*) and/or one integer SUM) */
     g.fused = 0; g.fused_cnt = -1; g.fused_sum = -1;

@@ -535,11 +535,6 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t phase) {
         : "memory");
   }
 }
-/* TMA bulk prefetch of a column slab into L2 (cp.async.bulk.prefetch.L2, SASS UBLKPF.L2): no registers, no shared
- * memory, one instruction per slab — the scan's loads then hit L2 (~300 cycles) instead of HBM (~800) */
-__device__ __forceinline__ void tma_prefetch_l2(const void* gsrc, uint32_t bytes) {
-  asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(gsrc), "r"(bytes) : "memory");
-}
 __device__ __forceinline__ void tma_bulk_g2s(void* smem_dst, const void* gsrc, uint32_t bytes, uint64_t* bar) {
   asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(smem_u32(smem_dst)),
                "l"(gsrc), "r"(bytes), "r"(smem_u32(bar))
@@ -554,8 +549,6 @@ struct ScanArgs {
   DevLaunch launch;
   SmemPlan smem;
   const int8_t* smem_image; /* identity image of ONE replica in HBM (MODE_SMEM) */
-  int32_t prefetch_distance; /* > 0: TMA bulk-prefetch the column slabs of the chunk this CTA will scan D iterations ahead into L2 */
-  int32_t pad_;
   int64_t ndv_bitmap_bytes;  /* estimator query: size of the ACC_NDV bitmap (a power of two) */
 };
 
@@ -1158,30 +1151,7 @@ __global__ void __launch_bounds__(BLOCK, 1024 / BLOCK) b2q_k_scan(const __grid_c
   int frag = 0;
   int64_t frag_first = 0;                                   /* first chunk of `frag` */
   int64_t next_first = __ldg(Lh.frag_chunk_start + 1);      /* first chunk of frag + 1 */
-  /* prefetch cursor (thread 0 only) */
-  const int pf_dist = A.prefetch_distance;
-  int pf_frag = 0;
-  int64_t pf_first = 0, pf_next = next_first;
   for (int64_t chunk = blockIdx.x; chunk < Lh.total_chunks; chunk += gridDim.x) {
-    if (pf_dist > 0 && tid == 0) {
-      const int64_t pc = chunk + (int64_t)pf_dist * gridDim.x;
-      if (pc < Lh.total_chunks) {
-        while (pc >= pf_next) {
-          ++pf_frag;
-          pf_first = pf_next;
-          pf_next = __ldg(Lh.frag_chunk_start + pf_frag + 1);
-        }
-        const int64_t prow = (pc - pf_first) * chunk_rows;
-        const int64_t pn = min(chunk_rows, __ldg(Lh.frag_rows + pf_frag) - prow);
-        const int8_t* const* pcols = Lh.col_ptrs + (size_t)pf_frag * P.n_cols;
-        for (int c = 0; c < P.n_cols; ++c) {
-          if (!P.col_prefetch[c]) continue;
-          const int w = P.col_width[c];
-          const uint32_t bytes = (uint32_t)(pn * w) & ~15u;
-          if (bytes) tma_prefetch_l2(pcols[c] + prow * w, bytes);
-        }
-      }
-    }
     while (chunk >= next_first) {
       ++frag;
       frag_first = next_first;
