@@ -43,13 +43,16 @@ ERR_CUDA = 1004
 ERR_KEY_OUT_OF_RANGE = 1005
 
 COMM_ID_BYTES = 128
-ABI_VERSION = 5   # B2Q_ABI_VERSION of include/b2q.h this mirror was written against
+ABI_VERSION = 6   # B2Q_ABI_VERSION of include/b2q.h this mirror was written against
 EXPR_COLUMN_VAR, EXPR_CONSTANT, EXPR_BIN_OPER, EXPR_AGG, EXPR_UOPER = 1, 2, 3, 4, 5
 CPU_LEVEL, GPU_LEVEL = 1, 2
 DEVICE_CPU, DEVICE_GPU = 0, 1
 KERNEL_AUTO, KERNEL_NON_GROUPED, KERNEL_PERFECT_SMEM, KERNEL_PERFECT_GLOBAL, KERNEL_BASELINE_GLOBAL, KERNEL_BASELINE_PROBE = range(6)
 DT_INT64, DT_FLOAT64, DT_UINT8 = 0, 1, 2
 RED_SUM, RED_MIN, RED_MAX, RED_BOR = 0, 1, 2, 3
+# b2q_rs_stat
+(STAT_FRAGMENTS_SCANNED, STAT_FRAGMENTS_SKIPPED, STAT_KERNEL_LAUNCHES, STAT_H2D_BYTES, STAT_SORT_US, STAT_HOST_SETUP_US,
+ STAT_HOST_STREAM_US, STAT_HOST_TEARDOWN_US, STAT_RESULT_D2H_BYTES) = range(9)
 
 MAX_SLOTS = 16
 MAX_TARGETS = 16
@@ -175,7 +178,7 @@ class ExecutionOptions(C.Structure):
         ("bigint_count", C.c_int32),
         ("force_kernel", C.c_int32),
         ("device_ordinal", C.c_int32),
-        ("pad_", C.c_int32),
+        ("result_on_device", C.c_int32),   # 1: the result stays in device memory until a host accessor needs it
     ]
 
 
@@ -264,6 +267,56 @@ class TargetValue(C.Structure):
         if self.is_null:
             return None
         return self.dval if self.is_fp else self.ival
+
+
+# ---- Arrow C Data / C Device Data Interface (include/b2q_arrow.h) -----------------------------------------------------
+ARROW_FLAG_NULLABLE = 2
+ARROW_DEVICE_CPU, ARROW_DEVICE_CUDA = 1, 2
+
+
+class ArrowSchema(C.Structure):
+    pass
+
+
+ArrowSchema._fields_ = [
+    ("format", C.c_char_p),
+    ("name", C.c_char_p),
+    ("metadata", C.c_char_p),
+    ("flags", C.c_int64),
+    ("n_children", C.c_int64),
+    ("children", C.POINTER(C.POINTER(ArrowSchema))),
+    ("dictionary", C.POINTER(ArrowSchema)),
+    ("release", C.CFUNCTYPE(None, C.POINTER(ArrowSchema))),
+    ("private_data", C.c_void_p),
+]
+
+
+class ArrowArray(C.Structure):
+    pass
+
+
+ArrowArray._fields_ = [
+    ("length", C.c_int64),
+    ("null_count", C.c_int64),
+    ("offset", C.c_int64),
+    ("n_buffers", C.c_int64),
+    ("n_children", C.c_int64),
+    ("buffers", C.POINTER(C.c_void_p)),
+    ("children", C.POINTER(C.POINTER(ArrowArray))),
+    ("dictionary", C.POINTER(ArrowArray)),
+    ("release", C.CFUNCTYPE(None, C.POINTER(ArrowArray))),
+    ("private_data", C.c_void_p),
+]
+
+
+class ArrowDeviceArray(C.Structure):
+    _fields_ = [
+        ("array", ArrowArray),
+        ("device_id", C.c_int64),
+        ("device_type", C.c_int32),
+        ("sync_event", C.c_void_p),   # ARROW_DEVICE_CUDA: a cudaEvent_t*
+        ("reserved", C.c_int64 * 3),
+    ]
 
 
 class Params(C.Structure):

@@ -8,7 +8,9 @@
  * warp-uniform, so the interpretation overhead is amortised and never diverges.
  */
 #pragma once
+#include <float.h>
 #include <stdint.h>
+#include <string.h>
 
 #include "../../include/b2q.h"
 
@@ -240,6 +242,154 @@ B2Q_HD int64_t b2q_acc_identity(int op) {
   }
 }
 
+/* ---- read-out of a reference-layout result buffer ------------------------------------------------------------
+ * One definition for the host reader (getNextRow / getRowAt / ColumnarResults in executor.cpp) and the device
+ * conversion (columnar.cu), so that the two cannot drift.  Slots are aligned to their padded width, so the device loads
+ * are plain typed loads; the host goes through memcpy. */
+#define B2Q_NULL_DOUBLE DBL_MIN
+#define B2Q_NULL_FLOAT FLT_MIN
+
+B2Q_HD int64_t b2q_ld(const int8_t* p, int w) {
+#if defined(__CUDA_ARCH__)
+  return w == 4 ? (int64_t)*reinterpret_cast<const int32_t*>(p) : *reinterpret_cast<const int64_t*>(p);
+#else
+  if (w == 4) { int32_t x; memcpy(&x, p, 4); return x; }
+  int64_t x;
+  memcpy(&x, p, 8);
+  return x;
+#endif
+}
+B2Q_HD float b2q_ld_f32(const int8_t* p) {
+#if defined(__CUDA_ARCH__)
+  return *reinterpret_cast<const float*>(p);
+#else
+  float f;
+  memcpy(&f, p, 4);
+  return f;
+#endif
+}
+B2Q_HD double b2q_bits_f64(int64_t bits) {
+#if defined(__CUDA_ARCH__)
+  return __longlong_as_double(bits);
+#else
+  double d;
+  memcpy(&d, &bits, 8);
+  return d;
+#endif
+}
+
+/* logical size / NULL sentinel (dictionary-encoded strings are int32 ids, TIME-family types int64) */
+B2Q_HD bool b2q_is_dict_string(int t) { return t == B2Q_kTEXT || t == B2Q_kVARCHAR || t == B2Q_kCHAR; }
+B2Q_HD bool b2q_is_decimal(int t) { return t == B2Q_kDECIMAL || t == B2Q_kNUMERIC; }
+B2Q_HD int b2q_type_size(int t) {
+  return t == B2Q_kTINYINT ? 1 : t == B2Q_kSMALLINT ? 2 : (t == B2Q_kINT || t == B2Q_kFLOAT || b2q_is_dict_string(t)) ? 4 : 8;
+}
+B2Q_HD int64_t b2q_int_null(int t) {
+  return t == B2Q_kTINYINT ? INT8_MIN : t == B2Q_kSMALLINT ? INT16_MIN : (t == B2Q_kINT || b2q_is_dict_string(t)) ? INT32_MIN : INT64_MIN;
+}
+B2Q_HD double b2q_exp_to_scale(int scale) { double d = 1; for (int i = 0; i < scale; ++i) d *= 10; return d; }
+
+/* where entry `e` keeps slot `s` / its first key: row-wise (ResultSet.h:55-70) or columnar (:72-84) */
+B2Q_HD const int8_t* b2q_slot_ptr(const B2QPlan& p, const int8_t* buf, int64_t e, int s) {
+  return p.output_columnar ? buf + p.slot_offset[s] + e * p.slot_padded_width[s] : buf + e * p.row_size + p.slot_offset[s];
+}
+B2Q_HD const int8_t* b2q_key_ptr(const B2QPlan& p, const int8_t* buf, int64_t e) {
+  return p.output_columnar ? buf + e * 8 : buf + e * p.row_size;
+}
+
+/* ResultSet::getColType: AVG reads as DOUBLE, every other target as its own type */
+B2Q_HD B2QTypeInfo b2q_target_col_type(const B2QTargetInfo& t) {
+  if (t.is_agg && t.agg_kind == B2Q_kAVG) { B2QTypeInfo d; d.type = B2Q_kDOUBLE; d.notnull = 0; d.scale = 0; return d; }
+  return t.sql_type;
+}
+
+/* getRowAt / getTargetValueFromBufferRowwise|Colwise (ResultSetIteration.cpp:820-1000) for target `i` of entry `entry` */
+B2Q_HD void b2q_read_target(const B2QPlan& p, const int8_t* buf, int64_t entry, int i, bool decimal_to_double, B2QTargetValue* out) {
+  const B2QTargetInfo& t = p.targets[i];
+  const int s = t.first_slot;
+  int w = p.slot_padded_width[s];
+  const int8_t* ptr = b2q_slot_ptr(p, buf, entry, s);
+  if (w == 0) { ptr = b2q_key_ptr(p, buf, entry); w = p.effective_key_width; } /* baseline: the key column is the target */
+  const int64_t ival = b2q_ld(ptr, w);
+  B2QTargetValue o;
+  o.is_fp = 0; o.is_null = 0; o.ival = 0; o.dval = 0;
+  /* compact type (get_compact_type): MIN/MAX -> argument type, otherwise the target type */
+  const bool has_arg = t.agg_arg_type.type != 0;
+  const int compact_type = (t.is_agg && has_arg && (t.agg_kind == B2Q_kMIN || t.agg_kind == B2Q_kMAX)) ? t.agg_arg_type.type : t.sql_type.type;
+  if (t.is_agg && t.agg_kind == B2Q_kAVG) { /* pair_to_double, ResultSetBufferAccessors.h:197-227 */
+    const int64_t cnt = b2q_ld(b2q_slot_ptr(p, buf, entry, s + 1), 8);
+    o.is_fp = 1;
+    if (cnt == 0) { o.dval = B2Q_NULL_DOUBLE; o.is_null = 1; }
+    else {
+      double dividend;
+      if (t.sql_type.type == B2Q_kDOUBLE) dividend = b2q_bits_f64(ival);
+      else if (t.sql_type.type == B2Q_kFLOAT) dividend = b2q_ld_f32(ptr); /* float_argument_input: pair_to_double reads the sum as a float */
+      else dividend = static_cast<double>(ival);
+      /* DECIMAL: one division by count x 10^scale, ResultSetBufferAccessors.h:222-225 */
+      o.dval = b2q_is_decimal(t.sql_type.type) && t.sql_type.scale ? dividend / (static_cast<double>(cnt) * b2q_exp_to_scale(t.sql_type.scale))
+                                                                   : dividend / static_cast<double>(cnt);
+      o.is_null = o.dval == B2Q_NULL_DOUBLE;
+    }
+  } else if (compact_type == B2Q_kDOUBLE) {
+    o.is_fp = 1;
+    o.dval = b2q_bits_f64(ival);
+    o.is_null = o.dval == B2Q_NULL_DOUBLE;
+  } else if (compact_type == B2Q_kFLOAT) { /* make_target_value: a float read from the slot's low 4 bytes (ResultSetIteration.cpp:2140-2160) */
+    const float f = b2q_ld_f32(ptr);
+    o.is_fp = 1;
+    o.dval = f;
+    o.is_null = f == B2Q_NULL_FLOAT;
+  } else if (b2q_is_decimal(compact_type)) { /* makeTargetValue, ResultSetIteration.cpp:2193-2210 */
+    const B2QTypeInfo& ct = compact_type == t.sql_type.type ? t.sql_type : t.agg_arg_type;
+    const bool agg_null = t.is_agg && (t.agg_kind == B2Q_kSUM || t.agg_kind == B2Q_kMIN || t.agg_kind == B2Q_kMAX);
+    o.is_null = ival == INT64_MIN && (agg_null || !ct.notnull);
+    if (decimal_to_double) {
+      o.is_fp = 1;
+      o.dval = o.is_null ? B2Q_NULL_DOUBLE : static_cast<double>(ival) / b2q_exp_to_scale(ct.scale);
+    } else o.ival = ival;
+  } else {
+    int64_t resized = ival;
+    switch (b2q_type_size(compact_type)) {
+      case 1: resized = static_cast<int8_t>(ival); break;
+      case 2: resized = static_cast<int16_t>(ival); break;
+      case 4: resized = static_cast<int32_t>(ival); break;
+      default: break;
+    }
+    if (resized == b2q_int_null(compact_type)) { o.ival = b2q_int_null(t.sql_type.type); o.is_null = 1; }
+    else o.ival = ival;
+  }
+  *out = o;
+}
+
+/* one value of a ColumnarResults column of byte width `width` (toBuffer, ColumnarResults.cpp:42-90); returns the
+ * stored bits widened to int64 (doubles / floats as their bit pattern) so that the caller can test them against the
+ * column's NULL sentinel */
+B2Q_HD int64_t b2q_store_target(const B2QTargetValue& v, int width, int8_t* dst) {
+  if (v.is_fp && width == 4) {
+    const float f = v.is_null ? B2Q_NULL_FLOAT : static_cast<float>(v.dval);
+    int32_t bits;
+    memcpy(&bits, &f, 4);
+    *reinterpret_cast<int32_t*>(dst) = bits;
+    return bits;
+  }
+  int64_t x = v.ival;
+  if (v.is_fp) memcpy(&x, &v.dval, 8);
+  switch (width) {
+    case 1: x = static_cast<int8_t>(x); *dst = static_cast<int8_t>(x); break;
+    case 2: x = static_cast<int16_t>(x); *reinterpret_cast<int16_t*>(dst) = static_cast<int16_t>(x); break;
+    case 4: x = static_cast<int32_t>(x); *reinterpret_cast<int32_t*>(dst) = static_cast<int32_t>(x); break;
+    default: *reinterpret_cast<int64_t*>(dst) = x;
+  }
+  return x;
+}
+
+/* the NULL sentinel of a ColumnarResults column as b2q_store_target returns its bits */
+B2Q_HD int64_t b2q_null_bits(int type) {
+  if (type == B2Q_kDOUBLE) { const double d = B2Q_NULL_DOUBLE; int64_t b; memcpy(&b, &d, 8); return b; }
+  if (type == B2Q_kFLOAT) { const float f = B2Q_NULL_FLOAT; int32_t b; memcpy(&b, &f, 4); return b; }
+  return b2q_int_null(type);
+}
+
 /* ---- launch description handed to the kernels ----------------------------------------------------------- */
 struct DevLaunch {
   /* column table: col_ptrs[frag * n_cols + c] — device pointers (device array) */
@@ -291,6 +441,22 @@ struct DevGatherCols {     /* columnar gather: every key / slot column, offsets 
   int64_t in_off[B2Q_MAX_SLOTS + B2Q_MAX_GROUP_COLS], out_off[B2Q_MAX_SLOTS + B2Q_MAX_GROUP_COLS];
   int8_t width[B2Q_MAX_SLOTS + B2Q_MAX_GROUP_COLS];
 };
+
+/* ---- device ColumnarResults (columnar.cu) over a result set of executor.cpp ----------------------------------- */
+namespace b2q {
+struct RsSource {
+  const B2QPlan* plan;
+  const int8_t* d_buf;  /* device copy of the storage (result_on_device), else nullptr */
+  const int8_t* h_buf;  /* host copy, else nullptr */
+  size_t buf_size;
+  int device;           /* device of d_buf, -1 without one */
+  const uint32_t* perm; /* ResultSet::permutation_ (host), n_perm entries; n_perm == 0: not sorted */
+  size_t n_perm;
+  size_t drop_first, keep_first;
+};
+bool rs_source(const B2QResultSet* rs, RsSource* out);
+DevSortLayout sort_layout_for(const B2QPlan& p);
+}  // namespace b2q
 
 /* host-side query object behind B2QQuery */
 struct B2QQuery {

@@ -386,6 +386,31 @@ namespace b2q {
 
 int sm_count();
 
+/* Step 1 on its own: the non-empty entries of `buf` in ascending order -> perm[0, *n_out).  block_counts holds
+ * ceil(entry_count / SORT_TILE) words, perm entry_count words; d_total is one device word.  One stream synchronisation
+ * (the count decides the caller's next allocation). */
+size_t compact_scratch_bytes(int64_t entries) {
+  const size_t n = (size_t)(entries > 0 ? entries : 1);
+  auto pad = [](size_t x) { return (x + 255) & ~size_t(255); };
+  return pad((n + SORT_TILE - 1) / SORT_TILE * 4) + pad(n * 4) + 256;
+}
+
+cudaError_t compact_entries(const DevSortLayout& L, const int8_t* buf, uint32_t* block_counts, uint32_t* perm, uint32_t* d_total,
+                            cudaStream_t st, int64_t* n_out) {
+  *n_out = 0;
+  if (L.entry_count <= 0) return cudaSuccess;
+  const int nblocks = (int)((L.entry_count + SORT_TILE - 1) / SORT_TILE);
+  b2q_k_sort_count<<<nblocks, SORT_BLOCK, 0, st>>>(L, buf, block_counts);
+  b2q_k_sort_scan<<<1, 1024, 0, st>>>(block_counts, (int64_t)nblocks, d_total);
+  b2q_k_sort_compact<<<nblocks, SORT_BLOCK, 0, st>>>(L, buf, block_counts, perm);
+  uint32_t h_total = 0;
+  cudaError_t e = cudaMemcpyAsync(&h_total, d_total, 4, cudaMemcpyDeviceToHost, st);
+  if (e == cudaSuccess) e = cudaStreamSynchronize(st);
+  if (e != cudaSuccess) return e;
+  *n_out = h_total;
+  return cudaSuccess;
+}
+
 /* Bytes of device scratch sort_device() needs for a table of `entries` entries. */
 size_t sort_scratch_bytes(int64_t entries) {
   const size_t n = (size_t)(entries > 0 ? entries : 1);
@@ -419,17 +444,11 @@ cudaError_t sort_device(const DevSortLayout& L, const DevSortKey* keys, int n_ke
   *n_out = 0;
   if (n_entries <= 0) return cudaSuccess;
 
-  b2q_k_sort_count<<<(int)nblocks_c, SORT_BLOCK, 0, st>>>(L, buf, block_counts);
-  b2q_k_sort_scan<<<1, 1024, 0, st>>>(block_counts, (int64_t)nblocks_c, d_total);
-  b2q_k_sort_compact<<<(int)nblocks_c, SORT_BLOCK, 0, st>>>(L, buf, block_counts, perm_a);
+  cudaError_t e = compact_entries(L, buf, block_counts, perm_a, d_total, st, n_out);
   *launches += 3;
+  if (e != cudaSuccess) return e;
   uint32_t h_total = 0;
-  cudaError_t e = cudaMemcpyAsync(&h_total, d_total, 4, cudaMemcpyDeviceToHost, st);
-  if (e != cudaSuccess) return e;
-  e = cudaStreamSynchronize(st);
-  if (e != cudaSuccess) return e;
-  int64_t n = h_total;
-  *n_out = n; /* the number of non-empty entries, whatever is sorted below */
+  int64_t n = *n_out; /* the number of non-empty entries, whatever is sorted below */
   if (n <= 1 || n_keys == 0) return cudaGetLastError();
 
   uint32_t* pin = perm_a;

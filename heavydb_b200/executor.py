@@ -152,6 +152,22 @@ def lib():
                                                   C.POINTER(C.POINTER(abi.TableInfo)), C.POINTER(abi.ExecUnit),
                                                   C.POINTER(abi.CompilationOptions), C.POINTER(abi.ExecutionOptions), C.c_int32,
                                                   C.POINTER(C.c_void_p)]
+        L.b2q_rs_device_columns.restype = C.c_int32
+        L.b2q_rs_device_columns.argtypes = [C.c_void_p, C.c_void_p, C.POINTER(C.c_void_p)]
+        for n in ("b2q_device_columns_size", "b2q_device_columns_num_columns"):
+            getattr(L, n).restype = C.c_size_t
+            getattr(L, n).argtypes = [C.c_void_p]
+        L.b2q_device_columns_device.restype = C.c_int32
+        L.b2q_device_columns_device.argtypes = [C.c_void_p]
+        L.b2q_device_columns_convert_ms.restype = C.c_double
+        L.b2q_device_columns_convert_ms.argtypes = [C.c_void_p]
+        L.b2q_device_columns_column.restype = C.c_void_p
+        L.b2q_device_columns_column.argtypes = [C.c_void_p, C.c_size_t, C.POINTER(abi.TypeInfo), C.POINTER(C.c_void_p),
+                                                C.POINTER(C.c_int64)]
+        L.b2q_device_columns_export_arrow.restype = C.c_int32
+        L.b2q_device_columns_export_arrow.argtypes = [C.c_void_p, C.POINTER(C.c_char_p), C.POINTER(abi.ArrowSchema),
+                                                      C.POINTER(abi.ArrowDeviceArray)]
+        L.b2q_device_columns_free.argtypes = [C.c_void_p, C.c_void_p]
         if L.b2q_abi_version() != abi.ABI_VERSION:
             raise ImportError("libb2q.so ABI version mismatch")
         _lib = L
@@ -176,8 +192,9 @@ def compilation_options(device_type: int = abi.DEVICE_GPU, hoist_literals: bool 
 
 
 def execution_options(allow_multifrag=True, output_columnar_hint=False, bigint_count=False, force_kernel=0,
-                      device_ordinal=-1) -> abi.ExecutionOptions:
+                      device_ordinal=-1, result_on_device=False) -> abi.ExecutionOptions:
     eo = abi.ExecutionOptions()
+    eo.result_on_device = int(result_on_device)
     eo.allow_multifrag = int(allow_multifrag)
     eo.output_columnar_hint = int(output_columnar_hint)
     eo.bigint_count = int(bigint_count)
@@ -265,7 +282,8 @@ class ResultSet:
         return {"fragments_scanned": L.b2q_rs_stat(self._h, 0), "fragments_skipped": L.b2q_rs_stat(self._h, 1),
                 "kernel_launches": L.b2q_rs_stat(self._h, 2), "h2d_bytes": L.b2q_rs_stat(self._h, 3),
                 "sort_us": L.b2q_rs_stat(self._h, 4), "host_setup_us": L.b2q_rs_stat(self._h, 5),
-                "host_stream_us": L.b2q_rs_stat(self._h, 6), "host_teardown_us": L.b2q_rs_stat(self._h, 7)}
+                "host_stream_us": L.b2q_rs_stat(self._h, 6), "host_teardown_us": L.b2q_rs_stat(self._h, 7),
+                "result_d2h_bytes": L.b2q_rs_stat(self._h, abi.STAT_RESULT_D2H_BYTES)}
 
     def columnarResults(self, num_threads: int = 8, with_scale: bool = False):
         """ColumnarResults(rows, num_columns, target_types) (QueryEngine/ColumnarResults.cpp:256-392): one numpy array per
@@ -313,6 +331,18 @@ class ResultSet:
         names = list(names) if names is not None else [f"col{i}" for i in range(len(arrays))]
         return pa.RecordBatch.from_arrays(arrays, names=names)
 
+    def deviceColumns(self, stream: Optional[int] = None) -> "DeviceColumns":
+        """The same columns as columnarResults(), made on the result's GPU (b2q_rs_device_columns): a result_on_device set is
+        read where it lies, without a device-to-host copy.  `stream`: the CUDA stream (handle as an int) the conversion is
+        ordered on; None = torch's current stream when torch is loaded, else the default stream."""
+        if stream is None:
+            stream = _current_torch_stream()
+        h = C.c_void_p()
+        rc = lib().b2q_rs_device_columns(self._h, C.c_void_p(stream), C.byref(h))
+        if rc:
+            _raise(rc)
+        return DeviceColumns(h, stream)
+
     def getNDVEstimator(self) -> int:
         """ResultSet::getNDVEstimator (CardinalityEstimator.cpp:33-52) of an estimator query."""
         return lib().b2q_rs_get_ndv_estimator(self._h)
@@ -338,6 +368,112 @@ class ResultSet:
 
     def keepFirstN(self, n: int):
         lib().b2q_rs_keep_first_n(self._h, n)
+
+
+def _current_torch_stream() -> int:
+    import sys
+    torch = sys.modules.get("torch")
+    if torch is None or not torch.cuda.is_initialized():
+        return 0
+    return int(torch.cuda.current_stream().cuda_stream)
+
+
+class _CudaArray:
+    """__cuda_array_interface__ (v3) over device memory a DeviceColumns owns; keeps that owner alive."""
+
+    def __init__(self, owner, ptr: int, n: int, typestr: str):
+        self._owner = owner
+        # "stream": None: b2q_rs_device_columns has completed the columns before it returned
+        self.__cuda_array_interface__ = {"shape": (n,), "typestr": typestr, "data": (ptr or 0, False), "version": 3,
+                                         "strides": None, "stream": None}
+
+
+class ArrowExport:
+    """An exported Arrow C Device record batch (ArrowSchema + ArrowDeviceArray): the ctypes structs, owned here until
+    release() (or garbage collection) calls their release callbacks."""
+
+    def __init__(self):
+        self.schema = abi.ArrowSchema()
+        self.array = abi.ArrowDeviceArray()
+
+    def release(self):
+        for obj in (self.array.array, self.schema):
+            if obj.release:
+                obj.release(C.byref(obj))
+
+    def __del__(self):
+        self.release()
+
+
+class DeviceColumns:
+    """ColumnarResults in device memory (b2q_rs_device_columns / b2q_device_columns_*): per target the values in the target
+    type's width (NULLs as the inline sentinel), an Arrow validity bitmap (None when the column has no NULL) and the NULL
+    count."""
+
+    def __init__(self, handle, stream: int = 0):
+        self._h = handle
+        self._stream = stream
+
+    def __del__(self):
+        if getattr(self, "_h", None):
+            lib().b2q_device_columns_free(self._h, C.c_void_p(self._stream))
+            self._h = None
+
+    def size(self) -> int:
+        return lib().b2q_device_columns_size(self._h)
+
+    def num_columns(self) -> int:
+        return lib().b2q_device_columns_num_columns(self._h)
+
+    def device(self) -> int:
+        return lib().b2q_device_columns_device(self._h)
+
+    def convert_ms(self) -> float:
+        """CUDA-event time of the conversion kernel."""
+        return lib().b2q_device_columns_convert_ms(self._h)
+
+    def column(self, i: int):
+        """(values device pointer, (sql_type, notnull, scale), validity device pointer or None, null_count)"""
+        ti, valid, nulls = abi.TypeInfo(), C.c_void_p(), C.c_int64()
+        ptr = lib().b2q_device_columns_column(self._h, i, C.byref(ti), C.byref(valid), C.byref(nulls))
+        if ptr is None and i >= self.num_columns():
+            raise IndexError(i)
+        return ptr or 0, (ti.type, bool(ti.notnull), ti.scale), valid.value, nulls.value
+
+    def tensors(self):
+        """[(values, validity)] as zero-copy CUDA torch tensors (validity: uint8 bitmap bytes, or None); they keep this
+        object — and so the device memory — alive."""
+        import torch
+        n = self.size()
+        out = []
+        for i in range(self.num_columns()):
+            ptr, (ty, _nn, _sc), valid, _nulls = self.column(i)
+            dev = torch.device("cuda", self.device())
+            vals = torch.as_tensor(_CudaArray(self, ptr, n, np.dtype(abi.NUMPY_OF[ty]).str), device=dev)
+            mask = torch.as_tensor(_CudaArray(self, valid, (n + 7) // 8, "|u1"), device=dev) if valid else None
+            out.append((vals, mask))
+        return out
+
+    def to_host(self):
+        """[(sql_type, notnull, values ndarray, validity bytes ndarray or None, null_count)] copied back to the host."""
+        out = []
+        for i, (vals, mask) in enumerate(self.tensors()):
+            _p, (ty, nn, _sc), _v, nulls = self.column(i)
+            out.append((ty, nn, vals.cpu().numpy(), None if mask is None else mask.cpu().numpy(), nulls))
+        return out
+
+    def export_arrow(self, names=None) -> ArrowExport:
+        """b2q_device_columns_export_arrow: the columns as an Arrow C Device record batch (a "+s" struct of one child per
+        target; device_type ARROW_DEVICE_CUDA).  The buffers stay alive until both this object and the export are released."""
+        ex = ArrowExport()
+        c_names = None
+        if names is not None:
+            ex._names = [str(x).encode() for x in names]
+            c_names = (C.c_char_p * len(ex._names))(*ex._names)
+        rc = lib().b2q_device_columns_export_arrow(self._h, c_names, C.byref(ex.schema), C.byref(ex.array))
+        if rc:
+            _raise(rc)
+        return ex
 
 
 class Partial:
@@ -436,9 +572,15 @@ class Executor:
 
     def executeWorkUnit(self, max_groups_buffer_entry_guess: int, is_agg: bool, query_infos, ra_exe_unit: abi.BuiltUnit,
                         co: Optional[abi.CompilationOptions] = None, eo: Optional[abi.ExecutionOptions] = None,
-                        has_cardinality_estimation: bool = False, memory_level: int = abi.CPU_LEVEL) -> ResultSet:
+                        has_cardinality_estimation: bool = False, memory_level: int = abi.CPU_LEVEL,
+                        result_on_device: Optional[bool] = None) -> ResultSet:
+        """result_on_device=True: the result stays in GPU memory (ResultSet.deviceColumns() reads it there; the first host
+        accessor copies it back once).  None keeps what `eo` says."""
         co = co or compilation_options()
         eo = eo or execution_options(device_ordinal=self.device_ordinal)
+        if result_on_device is not None:
+            eo = abi.ExecutionOptions.from_buffer_copy(eo)
+            eo.result_on_device = int(result_on_device)
         bt = self._built_table(query_infos, memory_level)
         guess = C.c_size_t(max_groups_buffer_entry_guess)
         h = C.c_void_p()

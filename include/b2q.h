@@ -37,13 +37,16 @@
 extern "C" {
 #endif
 
-#define B2Q_ABI_VERSION 5 /* 2: sort_info, join level, rte_idx, columnar, dictionary / time types, B2QPlan join fields;
+#define B2Q_ABI_VERSION 6 /* 2: sort_info, join level, rte_idx, columnar, dictionary / time types, B2QPlan join fields;
                             3: DATE_IN_DAYS chunks (negative col_encoded_sizes), column-vs-column quals, 16 filter leaves,
                                operands-before-node rule, b2q_columnar_results_*, host-phase stats;
                             4: DECIMAL / NUMERIC columns (B2QTypeInfo.scale), decimal_to_double of b2q_rs_get_next_row;
                             5: b2q_comm_* / b2q_execute_work_unit_dist / _multi (merge of the per-device tables inside the
                                library, NCCL), B2Q_KERNEL_BASELINE_PROBE, LIMIT 0 = empty result, COUNT(DISTINCT) on bitmaps
-                               (B2QPlan.count_distinct_*) */
+                               (B2QPlan.count_distinct_*);
+                            6: B2QExecutionOptions.result_on_device (was pad_), B2QDeviceColumns / b2q_rs_device_columns /
+                               b2q_device_columns_* (ColumnarResults in device memory, Arrow C Device export, b2q_arrow.h),
+                               B2Q_STAT_RESULT_D2H_BYTES */
 
 /* ---- SQLTypes subset (Shared/sqltypes.h:65-99) -------------------------------------------------------- */
 enum {
@@ -262,7 +265,11 @@ typedef struct B2QExecutionOptions {
   int32_t bigint_count;          /* g_bigint_count (--bigint-count) */
   int32_t force_kernel;          /* 0 = planner's choice; else B2Q_KERNEL_* (for tests / benchmarks) */
   int32_t device_ordinal;        /* CUDA device to run on (-1 = current); the calling thread's current device is restored on return */
-  int32_t pad_;
+  /* 1: the materialised result stays in device memory (no device-to-host copy inside the call); the host copy is made on the
+   * first host accessor of the result set (row_count, get_next_row, storage_buffer, columnar_results_create, ...), and
+   * b2q_rs_device_columns reads the device copy directly.  0 = copy the result to the host before returning.  Planning is
+   * the same either way; estimator results always come back to the host. */
+  int32_t result_on_device;
 } B2QExecutionOptions;
 
 /* static kernel families (one per C symbol b2q_k_*) */
@@ -504,7 +511,9 @@ void b2q_rs_keep_first_n(B2QResultSet* rs, size_t n);
 enum { B2Q_STAT_FRAGMENTS_SCANNED = 0, B2Q_STAT_FRAGMENTS_SKIPPED = 1 /* Executor::skipFragment, Execute.cpp:4776 */,
        B2Q_STAT_KERNEL_LAUNCHES = 2, B2Q_STAT_H2D_BYTES = 3, B2Q_STAT_SORT_US = 4 /* device time of compaction + sort + gather */,
        /* host wall-clock of the CPU_LEVEL streaming scan: staging setup, copy+scan pipeline, teardown */
-       B2Q_STAT_HOST_SETUP_US = 5, B2Q_STAT_HOST_STREAM_US = 6, B2Q_STAT_HOST_TEARDOWN_US = 7 };
+       B2Q_STAT_HOST_SETUP_US = 5, B2Q_STAT_HOST_STREAM_US = 6, B2Q_STAT_HOST_TEARDOWN_US = 7,
+       B2Q_STAT_RESULT_D2H_BYTES = 8 /* result-storage bytes copied device -> host so far (0 for a result_on_device set no host
+                                        accessor has read yet) */ };
 int64_t b2q_rs_stat(const B2QResultSet* rs, int32_t which);
 void b2q_rs_free(B2QResultSet* rs);
 /* ResultSet(targets, device_type, query_mem_desc, ...) + allocateStorage(buffer) (ResultSet.h:183-217): a result set over a
@@ -512,6 +521,36 @@ void b2q_rs_free(B2QResultSet* rs);
  * copied.  Read-out only (rowCount / getNextRow / isRowAtEmpty / ColumnarResults) — nothing is computed and no device is
  * needed, the way ResultSetTest wraps hand-filled storage. */
 int32_t b2q_rs_create_from_storage(const B2QQuery* q, const int8_t* storage, size_t size_bytes, B2QResultSet** out);
+
+/* ---- ColumnarResults in device memory ------------------------------------------------------------------------
+ * b2q_rs_device_columns converts a result set, on `cuda_stream` of the result's device, into exactly what
+ * b2q_columnar_results_create produces on the host: the same rows in iteration order (permutation, OFFSET, LIMIT applied),
+ * one array per target in the target type's width, NULLs as the inline sentinel.  A result_on_device set is read where it
+ * lies (no device-to-host copy); a host-resident one is uploaded first.  Each column also gets an Arrow validity bitmap
+ * (bit set = valid, LSB first, one bit per row) and its NULL count; a column without NULLs reports validity = NULL and
+ * null_count = 0.  Returns once the columns are complete.  Without a CUDA device: B2Q_ERR_NO_DEVICE.
+ *
+ * b2q_device_columns_export_arrow fills an Arrow C Device Data Interface record batch (b2q_arrow.h): a "+s" struct with
+ * one child per target, formats c/s/i/l/f/g (dictionary ids i, TIME-family l) and d:19,<scale> for DECIMAL (a decimal128
+ * buffer made on the device), device_type ARROW_DEVICE_CUDA, device_id = the result's device, sync_event -> a cudaEvent_t
+ * recorded after the conversion.  `names` may be NULL ("col<i>").  The buffers stay alive until both
+ * b2q_device_columns_free and the exported array's release have run; whichever runs last frees them stream-ordered
+ * (b2q_device_columns_free on its `cuda_stream`; release on the legacy default stream after the conversion's event, i.e.
+ * after work the consumer enqueued on any blocking stream of that device). */
+typedef struct B2QDeviceColumns B2QDeviceColumns;
+struct ArrowSchema;
+struct ArrowDeviceArray;
+int32_t b2q_rs_device_columns(const B2QResultSet* rs, void* cuda_stream, B2QDeviceColumns** out);
+size_t b2q_device_columns_size(const B2QDeviceColumns* dc);        /* rows */
+size_t b2q_device_columns_num_columns(const B2QDeviceColumns* dc);
+int32_t b2q_device_columns_device(const B2QDeviceColumns* dc);     /* CUDA device ordinal of the buffers */
+double b2q_device_columns_convert_ms(const B2QDeviceColumns* dc);  /* CUDA-event time of the conversion kernel */
+/* device pointer of column `col`'s values (NULL for an index out of range); *validity = its bitmap or NULL */
+const void* b2q_device_columns_column(const B2QDeviceColumns* dc, size_t col, B2QTypeInfo* type_info, const uint32_t** validity,
+                                      int64_t* null_count);
+int32_t b2q_device_columns_export_arrow(B2QDeviceColumns* dc, const char* const* names, struct ArrowSchema* schema,
+                                        struct ArrowDeviceArray* array);
+void b2q_device_columns_free(B2QDeviceColumns* dc, void* cuda_stream);
 
 /* ---- synthetic data (bench / tests): counter-based generator, identical to oracle/oracle_gen.h ----------
  * value(row) = lo + splitmix64(seed ^ (col_tag << 56) ^ row) % span   (integers)

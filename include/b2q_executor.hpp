@@ -23,6 +23,7 @@
 #include <vector>
 
 #include "b2q.h"
+#include "b2q_arrow.h"
 
 namespace b2q {
 
@@ -175,6 +176,7 @@ struct ExecutionOptions { /* CompilationOptions.h:70-122 */
   bool allow_multifrag{true};
   bool output_columnar_hint{false};
   bool bigint_count{false}; /* g_bigint_count */
+  bool result_on_device{false}; /* keep the result in device memory (B2QExecutionOptions::result_on_device) */
   static ExecutionOptions defaults() { return ExecutionOptions{}; }
 };
 struct RenderInfo;              /* unused on this path */
@@ -255,6 +257,51 @@ class ColumnarResults {
  private:
   B2QColumnarResults* h_{nullptr};
   std::vector<const int8_t*> column_buffers_;
+  std::vector<SQLTypeInfo> target_types_;
+};
+
+/* The same columns in device memory (b2q_rs_device_columns): what the GPU branch of ArrowResultSetConverter hands over.
+ * Column buffers, validity bitmaps (nullptr for a column without NULLs) and NULL counts live as long as this object, or as
+ * long as an Arrow export of it that has not been released, whichever is longer. */
+class DeviceColumnarResults {
+ public:
+  explicit DeviceColumnarResults(const ResultSet& rows, void* cuda_stream = nullptr) : stream_(cuda_stream) {
+    const int32_t rc = b2q_rs_device_columns(rows.handle(), cuda_stream, &h_);
+    if (rc != B2Q_OK) throw QueryExecutionError(rc, b2q_last_error_message());
+    const size_t nc = b2q_device_columns_num_columns(h_);
+    for (size_t c = 0; c < nc; ++c) {
+      B2QTypeInfo ti;
+      const uint32_t* valid = nullptr;
+      int64_t nulls = 0;
+      column_buffers_.push_back(static_cast<const int8_t*>(b2q_device_columns_column(h_, c, &ti, &valid, &nulls)));
+      validity_.push_back(valid);
+      null_counts_.push_back(nulls);
+      target_types_.emplace_back(static_cast<SQLTypes>(ti.type), ti.notnull != 0);
+      target_types_.back().scale = ti.scale;
+    }
+  }
+  ~DeviceColumnarResults() { b2q_device_columns_free(h_, stream_); }
+  DeviceColumnarResults(const DeviceColumnarResults&) = delete;
+  DeviceColumnarResults& operator=(const DeviceColumnarResults&) = delete;
+  const std::vector<const int8_t*>& getColumnBuffers() const { return column_buffers_; } /* device pointers */
+  const std::vector<const uint32_t*>& getValidityBitmaps() const { return validity_; }
+  int64_t nullCount(const int col_id) const { return null_counts_[col_id]; }
+  size_t size() const { return b2q_device_columns_size(h_); }
+  int deviceId() const { return b2q_device_columns_device(h_); }
+  const SQLTypeInfo& getColumnType(const int col_id) const { return target_types_[col_id]; }
+  /* Arrow C Device Data Interface record batch; the caller owns both structs and calls their release */
+  void exportArrow(const std::vector<std::string>& names, ArrowSchema* schema, ArrowDeviceArray* array) const {
+    std::vector<const char*> cn;
+    for (const auto& n : names) cn.push_back(n.c_str());
+    const int32_t rc = b2q_device_columns_export_arrow(h_, cn.empty() ? nullptr : cn.data(), schema, array);
+    if (rc != B2Q_OK) throw QueryExecutionError(rc, b2q_last_error_message());
+  }
+ private:
+  void* stream_;
+  B2QDeviceColumns* h_{nullptr};
+  std::vector<const int8_t*> column_buffers_;
+  std::vector<const uint32_t*> validity_;
+  std::vector<int64_t> null_counts_;
   std::vector<SQLTypeInfo> target_types_;
 };
 
@@ -351,7 +398,8 @@ class Executor {
     u.offset = static_cast<int64_t>(ra_exe_unit.sort_info.offset);
     u.has_window_function = ra_exe_unit.has_window_function;
     B2QCompilationOptions cco{static_cast<int32_t>(co.device_type), co.hoist_literals ? 1 : 0, co.filter_on_deleted_column ? 0 : 1, 0};
-    B2QExecutionOptions ceo{options.allow_multifrag ? 1 : 0, options.output_columnar_hint ? 1 : 0, options.bigint_count ? 1 : 0, 0, -1, 0};
+    B2QExecutionOptions ceo{options.allow_multifrag ? 1 : 0, options.output_columnar_hint ? 1 : 0, options.bigint_count ? 1 : 0, 0, -1,
+                            options.result_on_device ? 1 : 0};
     B2QResultSet* rs = nullptr;
     int32_t rc;
     if (storage) {
