@@ -43,7 +43,7 @@ ERR_CUDA = 1004
 ERR_KEY_OUT_OF_RANGE = 1005
 
 COMM_ID_BYTES = 128
-ABI_VERSION = 6   # B2Q_ABI_VERSION of include/b2q.h this mirror was written against
+ABI_VERSION = 7   # B2Q_ABI_VERSION of include/b2q.h this mirror was written against
 EXPR_COLUMN_VAR, EXPR_CONSTANT, EXPR_BIN_OPER, EXPR_AGG, EXPR_UOPER = 1, 2, 3, 4, 5
 CPU_LEVEL, GPU_LEVEL = 1, 2
 DEVICE_CPU, DEVICE_GPU = 0, 1
@@ -52,7 +52,7 @@ DT_INT64, DT_FLOAT64, DT_UINT8 = 0, 1, 2
 RED_SUM, RED_MIN, RED_MAX, RED_BOR = 0, 1, 2, 3
 # b2q_rs_stat
 (STAT_FRAGMENTS_SCANNED, STAT_FRAGMENTS_SKIPPED, STAT_KERNEL_LAUNCHES, STAT_H2D_BYTES, STAT_SORT_US, STAT_HOST_SETUP_US,
- STAT_HOST_STREAM_US, STAT_HOST_TEARDOWN_US, STAT_RESULT_D2H_BYTES) = range(9)
+ STAT_HOST_STREAM_US, STAT_HOST_TEARDOWN_US, STAT_RESULT_D2H_BYTES, STAT_ROWS_SCANNED) = range(10)
 
 MAX_SLOTS = 16
 MAX_TARGETS = 16

@@ -35,7 +35,7 @@ CXX_FLAGS = ["-O2", "-std=c++17", "-fPIC", "-Wall", "-Wno-unused-function", "-pt
 # (unit name, source file, extra defines).  scan_inst.cu holds the b2q_k_scan instantiations of one
 # (join level, table-mode group); nine units so that they compile in parallel.
 UNITS = [(f"scan_j{j}_g{g}", "scan_inst.cu", [f"-DB2Q_SCAN_JOIN={j}", f"-DB2Q_SCAN_GROUP={g}"]) for j in range(3) for g in range(3)]
-UNITS += [("kernels", "kernels.cu", []), ("sort", "sort.cu", []), ("radix_agg", "radix_agg.cu", []), ("columnar", "columnar.cu", []),
+UNITS += [("kernels", "kernels.cu", []), ("sort", "sort.cu", []), ("radix_agg", "radix_agg.cu", []), ("columnar", "columnar.cu", []), ("project", "project.cu", []),
           ("executor", "executor.cpp", []), ("multi", "multi.cpp", []), ("planner", "planner.cpp", [])]
 
 

@@ -250,9 +250,12 @@ B2Q_HD int64_t b2q_acc_identity(int op) {
 #define B2Q_NULL_FLOAT FLT_MIN
 
 B2Q_HD int64_t b2q_ld(const int8_t* p, int w) {
+  if (w == 1) return *p; /* projection: logical-sized TINYINT / SMALLINT columns of a columnar buffer */
 #if defined(__CUDA_ARCH__)
+  if (w == 2) return *reinterpret_cast<const int16_t*>(p);
   return w == 4 ? (int64_t)*reinterpret_cast<const int32_t*>(p) : *reinterpret_cast<const int64_t*>(p);
 #else
+  if (w == 2) { int16_t x; memcpy(&x, p, 2); return x; }
   if (w == 4) { int32_t x; memcpy(&x, p, 4); return x; }
   int64_t x;
   memcpy(&x, p, 8);
@@ -458,6 +461,27 @@ bool rs_source(const B2QResultSet* rs, RsSource* out);
 DevSortLayout sort_layout_for(const B2QPlan& p);
 }  // namespace b2q
 
+/* ---- projection (project.cu): one projected column, decoded the way the chunk decoders hand it to agg_id ----------- */
+enum { PROJ_INT = 0, PROJ_F64 = 1, PROJ_F32 = 2 };
+struct DevProjCol {
+  int64_t null_phys;    /* the chunk's NULL as loaded (sign-extended; 255 / 65535 for DICT(8|16)) */
+  int64_t null_logical; /* what a NULL row stores: the logical type's sentinel */
+  int64_t out_off;      /* row-wise: byte offset inside the row; columnar: offset of the column */
+  int32_t col;          /* launch column */
+  int8_t width;         /* physical width code of the chunk (load32 / load64) */
+  int8_t out_w;         /* slot width: 8 row-wise, the logical size columnar */
+  int8_t kind;          /* PROJ_* */
+  int8_t days;          /* DATE ENCODING DAYS: value * 86400 */
+  int8_t translate_null;/* the physical NULL differs from the logical one (ENCODING FIXED, DICT(8|16), DAYS) */
+  int8_t pad_[7];
+};
+struct DevProject {
+  int32_t n;
+  int32_t pad_;
+  int64_t scan_limit;   /* B2QExecUnit::scan_limit (0 = none) */
+  DevProjCol cols[B2Q_MAX_TARGETS];
+};
+
 /* host-side query object behind B2QQuery */
 struct B2QQuery {
   B2QPlan plan;
@@ -474,4 +498,5 @@ struct B2QQuery {
   int32_t has_limit;
   int64_t limit, offset;
   int64_t total_tuples;          /* rows of all fragments of the table (every device's) */
+  DevProject proj;               /* plan.query_desc_type == B2Q_Projection */
 };

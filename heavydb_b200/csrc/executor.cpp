@@ -55,6 +55,11 @@ cudaError_t sort_device(const DevSortLayout& L, const DevSortKey* keys, int n_ke
                         cudaStream_t st, const uint32_t** perm_out, int64_t* n_out, int* launches, int64_t top_n);
 cudaError_t sort_gather(const DevSortLayout& Lin, const DevGatherCols& G, const int8_t* in, int8_t* out, const uint32_t* perm,
                         int64_t first, int64_t n_out, cudaStream_t st);
+int project_rows_per_chunk();
+cudaError_t launch_project(const B2QQuery& q, const int8_t* const* col_ptrs, const int64_t* frag_rows, const int64_t* frag_chunk_start,
+                           const int64_t* frag_row_base, int n_frags, int64_t total_chunks, int64_t chunk_base, int8_t* out,
+                           int64_t row_size, int64_t cap, unsigned long long* status, unsigned long long* ticket,
+                           unsigned long long* counters, cudaStream_t st);
 }  // namespace b2q
 
 using namespace b2q;
@@ -260,6 +265,7 @@ struct B2QResultSet {
   double scan_ms = 0, init_ms = 0, mat_ms = 0, h2d_bytes = 0;
   double host_setup_us = 0, host_stream_us = 0, host_teardown_us = 0;
   int64_t launches = 0, frags_scanned = 0, frags_skipped = 0;
+  int64_t rows_scanned = 0; /* B2Q_STAT_ROWS_SCANNED */
   bool heap_buf = false; /* b2q_rs_create_from_storage: a plain heap copy of the caller's buffer (no device involved) */
   ~B2QResultSet() {
     if (heap_buf) free(buf); else pinned_cache().put(buf, buf_cap);
@@ -801,6 +807,8 @@ static int32_t execute_partial_attempt(size_t* guess, const B2QTableInfo* tbl, c
   const size_t g = guess ? *guess : 0;
   int32_t rc = make_query(u, tbl, eo, g, has_card != 0, !co->ignore_deleted_column, &p->q, &err);
   if (rc != B2Q_OK) return set_err(rc, err);
+  if (p->q.plan.query_desc_type == B2Q_Projection)
+    return set_err(B2Q_ERR_UNSUPPORTED, "projection units run through b2q_execute_work_unit (one device); the split and multi-device forms are outside this path");
   g_trace.mark("plan");
   if (!have_device()) return set_err(B2Q_ERR_NO_DEVICE, "no CUDA device visible; this path has no CPU fallback");
   if (eo->device_ordinal >= 0) CU(cudaSetDevice(eo->device_ordinal));
@@ -961,6 +969,62 @@ static void limit_window(const B2QQuery& q, int64_t n, int64_t* first, int64_t* 
   *count = c;
 }
 
+/* ORDER BY / LIMIT / OFFSET over a materialised device buffer laid out as rs->q.plan says: compaction of the non-empty
+ * entries, sort, and a gather of the kept rows into a compact buffer, which becomes the result (rs->d_buf when on_device,
+ * else copied into rs->buf).  Frees d_in (stream-ordered) and returns after the stream's work is complete. */
+static int32_t sort_keep_rows(B2QResultSet* rs, int8_t* d_in, bool on_device, int device, cudaStream_t st) {
+  const B2QPlan plan = rs->q.plan;
+  const B2QQuery& q = rs->q;
+  int8_t* d_scratch = nullptr;
+  int8_t* d_compact = nullptr;
+  cudaError_t e = cudaMallocAsync(reinterpret_cast<void**>(&d_scratch), sort_scratch_bytes(plan.entry_count), st);
+  cudaEvent_t ev0 = nullptr, ev1 = nullptr;
+  cudaEventCreate(&ev0); cudaEventCreate(&ev1);
+  const DevSortLayout L = sort_layout_of(plan);
+  DevSortKey keys[B2Q_MAX_ORDER_ENTRIES];
+  for (int i = 0; i < q.n_order; ++i) keys[i] = sort_key_of(plan, q.order[i]);
+  const uint32_t* d_perm = nullptr;
+  int64_t n = 0, first = 0, count = 0;
+  int sort_launches = 0;
+  if (e == cudaSuccess) e = cudaEventRecord(ev0, st);
+  if (e == cudaSuccess) e = sort_device(L, keys, q.n_order, d_in, d_scratch, st, &d_perm, &n, &sort_launches,
+                                        (q.has_limit ? q.limit : 0) + q.offset);
+  if (e == cudaSuccess) {
+    limit_window(q, n, &first, &count);
+    relayout_entries(rs->q.plan, count);
+    rs->buf_size = static_cast<size_t>(rs->q.plan.buffer_size);
+    if (rs->buf_size) {
+      if (!on_device) {
+        rs->buf = pinned_cache().get(rs->buf_size, &rs->buf_cap);
+        if (!rs->buf) e = cudaErrorMemoryAllocation;
+      }
+      if (e == cudaSuccess) e = cudaMallocAsync(reinterpret_cast<void**>(&d_compact), rs->buf_size, st);
+      const DevGatherCols G = gather_cols_of(plan, rs->q.plan);
+      if (e == cudaSuccess) e = sort_gather(L, G, d_in, d_compact, d_perm, first, count, st);
+      if (e == cudaSuccess) e = cudaEventRecord(ev1, st);
+      if (on_device) { /* the compact buffer IS the result */
+        if (e == cudaSuccess) { rs->d_buf = d_compact; rs->device = device; d_compact = nullptr; }
+      } else if (e == cudaSuccess) {
+        e = cudaMemcpyAsync(rs->buf, d_compact, rs->buf_size, cudaMemcpyDeviceToHost, st);
+        rs->d2h_bytes = static_cast<int64_t>(rs->buf_size);
+      }
+      sort_launches += 1;
+    } else if (e == cudaSuccess) {
+      e = cudaEventRecord(ev1, st);
+    }
+  }
+  if (d_compact) cudaFreeAsync(d_compact, st);
+  if (d_scratch) cudaFreeAsync(d_scratch, st);
+  cudaFreeAsync(d_in, st);
+  if (e == cudaSuccess) e = cudaStreamSynchronize(st);
+  if (e == cudaSuccess) { float ms = 0; if (cudaEventElapsedTime(&ms, ev0, ev1) == cudaSuccess) rs->sort_ms = ms; }
+  cudaEventDestroy(ev0); cudaEventDestroy(ev1);
+  if (e != cudaSuccess) { cudaGetLastError(); return set_err(B2Q_ERR_CUDA, std::string("sort/materialise: ") + cudaGetErrorString(e)); }
+  rs->sorted = true;
+  rs->launches += sort_launches;
+  return B2Q_OK;
+}
+
 static int32_t finalize_core(B2QPartial* p, cudaStream_t st, B2QResultSet** out);
 
 static int32_t finalize_impl(B2QPartial* p, cudaStream_t st, B2QResultSet** out) {
@@ -1011,57 +1075,12 @@ static int32_t finalize_core(B2QPartial* p, cudaStream_t st, B2QResultSet** out)
   const bool want_sort = p->q.n_order > 0 || p->q.has_limit || p->q.offset > 0;
   if (nbytes && want_sort) {
     /* materialise on the device, sort / truncate there, copy back only the kept rows */
-    const B2QPlan& plan = p->q.plan;
     int8_t* d_out = nullptr;
-    int8_t* d_scratch = nullptr;
-    int8_t* d_compact = nullptr;
     CU(cudaMallocAsync(reinterpret_cast<void**>(&d_out), nbytes, st));
     cudaError_t e = launch_materialize(p->q, p->accs, p->keys, d_out, st);
-    if (e == cudaSuccess) e = cudaMallocAsync(reinterpret_cast<void**>(&d_scratch), sort_scratch_bytes(plan.entry_count), st);
-    cudaEvent_t ev0 = nullptr, ev1 = nullptr;
-    cudaEventCreate(&ev0); cudaEventCreate(&ev1);
-    const DevSortLayout L = sort_layout_of(plan);
-    DevSortKey keys[B2Q_MAX_ORDER_ENTRIES];
-    for (int i = 0; i < p->q.n_order; ++i) keys[i] = sort_key_of(plan, p->q.order[i]);
-    const uint32_t* d_perm = nullptr;
-    int64_t n = 0, first = 0, count = 0;
-    int sort_launches = 0;
-    if (e == cudaSuccess) e = cudaEventRecord(ev0, st);
-    if (e == cudaSuccess) e = sort_device(L, keys, p->q.n_order, d_out, d_scratch, st, &d_perm, &n, &sort_launches,
-                                          (p->q.has_limit ? p->q.limit : 0) + p->q.offset);
-    if (e == cudaSuccess) {
-      limit_window(p->q, n, &first, &count);
-      relayout_entries(rs->q.plan, count);
-      rs->buf_size = static_cast<size_t>(rs->q.plan.buffer_size);
-      if (rs->buf_size) {
-        if (!p->result_on_device) {
-          rs->buf = pinned_cache().get(rs->buf_size, &rs->buf_cap);
-          if (!rs->buf) e = cudaErrorMemoryAllocation;
-        }
-        if (e == cudaSuccess) e = cudaMallocAsync(reinterpret_cast<void**>(&d_compact), rs->buf_size, st);
-        const DevGatherCols G = gather_cols_of(plan, rs->q.plan);
-        if (e == cudaSuccess) e = sort_gather(L, G, d_out, d_compact, d_perm, first, count, st);
-        if (e == cudaSuccess) e = cudaEventRecord(ev1, st);
-        if (p->result_on_device) { /* the compact buffer IS the result */
-          if (e == cudaSuccess) { rs->d_buf = d_compact; rs->device = p->device; d_compact = nullptr; }
-        } else if (e == cudaSuccess) {
-          e = cudaMemcpyAsync(rs->buf, d_compact, rs->buf_size, cudaMemcpyDeviceToHost, st);
-          rs->d2h_bytes = static_cast<int64_t>(rs->buf_size);
-        }
-        sort_launches += 1;
-      } else if (e == cudaSuccess) {
-        e = cudaEventRecord(ev1, st);
-      }
-    }
-    if (d_compact) cudaFreeAsync(d_compact, st);
-    if (d_scratch) cudaFreeAsync(d_scratch, st);
-    cudaFreeAsync(d_out, st);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(st);
-    if (e == cudaSuccess) { float ms = 0; if (cudaEventElapsedTime(&ms, ev0, ev1) == cudaSuccess) rs->sort_ms = ms; }
-    cudaEventDestroy(ev0); cudaEventDestroy(ev1);
-    if (e != cudaSuccess) { cudaGetLastError(); return set_err(B2Q_ERR_CUDA, std::string("sort/materialise: ") + cudaGetErrorString(e)); }
-    rs->sorted = true;
-    rs->launches += sort_launches;
+    if (e != cudaSuccess) { cudaFreeAsync(d_out, st); cudaGetLastError(); return set_err(B2Q_ERR_CUDA, std::string("materialise: ") + cudaGetErrorString(e)); }
+    const int32_t rc = sort_keep_rows(rs.get(), d_out, p->result_on_device, p->device, st);
+    if (rc != B2Q_OK) return rc;
     *out = rs.release();
     return B2Q_OK;
   }
@@ -1229,6 +1248,337 @@ static int32_t execute_work_unit_rank(const B2QComm* comm, size_t* guess, const 
   return set_err(B2Q_ERR_CUDA, "internal: radix retry did not converge");
 }
 
+/* ---- projection (project.cu) ---------------------------------------------------------------------------------------
+ * One launch of b2q_k_project over `nf` fragments whose referenced columns are in device memory, writing at most `cap` rows
+ * into `d_out` (laid out for `cap` entries).  Returns the rows written and the rows of the chunks the kernel loaded after
+ * the call's host wait. */
+struct ProjectRun {
+  int64_t written = 0, scanned = 0;
+  double kernel_ms = 0;
+};
+static int32_t project_scan(const B2QQuery& q, int nf, const std::vector<const int8_t*>& cols, const std::vector<int64_t>& rows,
+                            int8_t* d_out, int64_t cap, cudaStream_t st, ProjectRun* run) {
+  const int64_t chunk_rows = project_rows_per_chunk();
+  const int nc = q.prog.n_cols;
+  std::vector<int64_t> host(static_cast<size_t>(nf) * nc + nf + nf + 1);
+  memcpy(host.data(), cols.data(), static_cast<size_t>(nf) * nc * 8);
+  int64_t* h_rows = host.data() + static_cast<size_t>(nf) * nc;
+  int64_t* cs = h_rows + nf;
+  cs[0] = 0;
+  for (int f = 0; f < nf; ++f) { h_rows[f] = rows[f]; cs[f + 1] = cs[f] + (rows[f] + chunk_rows - 1) / chunk_rows; }
+  const int64_t chunks = cs[nf];
+  run->written = run->scanned = 0;
+  if (chunks == 0 || cap == 0) return B2Q_OK;
+  const size_t tab_bytes = DeviceBlock::pad(host.size() * 8), status_bytes = DeviceBlock::pad(static_cast<size_t>(chunks) * 8);
+  int8_t* blk = nullptr;
+  CU(cudaMallocAsync(reinterpret_cast<void**>(&blk), tab_bytes + status_bytes + 256, st));
+  unsigned long long* status = reinterpret_cast<unsigned long long*>(blk + tab_bytes);
+  unsigned long long* counters = reinterpret_cast<unsigned long long*>(blk + tab_bytes + status_bytes); /* ticket, done, written, scanned */
+  unsigned long long h_counters[4] = {};
+  cudaEvent_t ev[2] = {};
+  cudaError_t e = cudaMemcpyAsync(blk, host.data(), host.size() * 8, cudaMemcpyHostToDevice, st);
+  if (e == cudaSuccess) e = cudaMemsetAsync(status, 0, status_bytes + 256, st);
+  if (e == cudaSuccess) e = cudaEventCreate(&ev[0]);
+  if (e == cudaSuccess) e = cudaEventCreate(&ev[1]);
+  if (e == cudaSuccess) e = cudaEventRecord(ev[0], st);
+  if (e == cudaSuccess) {
+    const int8_t* const* d_cols = reinterpret_cast<const int8_t* const*>(blk);
+    const int64_t* d_rows = reinterpret_cast<const int64_t*>(blk) + static_cast<size_t>(nf) * nc;
+    const int64_t row_size = q.plan.output_columnar ? 0 : q.plan.row_size;
+    e = launch_project(q, d_cols, d_rows, d_rows + nf, nullptr, nf, chunks, 0, d_out, row_size, cap, status, counters, counters + 1, st);
+  }
+  if (e == cudaSuccess) e = cudaEventRecord(ev[1], st);
+  if (e == cudaSuccess) e = cudaMemcpyAsync(h_counters, counters, sizeof(h_counters), cudaMemcpyDeviceToHost, st);
+  cudaFreeAsync(blk, st);
+  if (e == cudaSuccess) e = cudaStreamSynchronize(st);
+  float ms = 0;
+  if (e == cudaSuccess && cudaEventElapsedTime(&ms, ev[0], ev[1]) == cudaSuccess) run->kernel_ms = ms;
+  for (cudaEvent_t x : ev) if (x) cudaEventDestroy(x);
+  if (e != cudaSuccess) { cudaGetLastError(); return set_err(e == cudaErrorMemoryAllocation ? B2Q_ERR_OUT_OF_GPU_MEM : B2Q_ERR_CUDA, std::string("projection: ") + cudaGetErrorString(e)); }
+  run->written = static_cast<int64_t>(h_counters[2]);
+  run->scanned = static_cast<int64_t>(h_counters[3]);
+  return B2Q_OK;
+}
+
+/* The same over a host-resident table: the referenced columns stream through two staging buffer sets in slices of 16 Mi rows,
+ * the copy of slice k+1 overlapping the scan of slice k, one launch per slice.  The launches continue one order: the status
+ * words are indexed by a chunk number that runs on across slices (chunk_base), every slice has its own ticket, the done flag
+ * and the row counters are shared, and each slice's offset words start at its first row in the fragment.  Before a staging set
+ * is reused the host reads the done flag as of the scan that last used it, so a scan limit also stops the copies. */
+static int32_t project_scan_host(const B2QQuery& q, const B2QTableInfo& tbl, const std::vector<int>& frags, int8_t* d_out, int64_t cap,
+                                 cudaStream_t st, ProjectRun* run, double* h2d_bytes) {
+  const int64_t chunk_rows = project_rows_per_chunk();
+  const int64_t slice_rows = int64_t(1) << 24; /* a multiple of chunk_rows */
+  const int nc = q.prog.n_cols;
+  struct Slice { int frag; int64_t row0, rows, chunk_base; };
+  std::vector<Slice> sl;
+  int64_t chunks = 0, max_rows = 0;
+  for (int f : frags)
+    for (int64_t r = 0; r < tbl.fragments[f].num_tuples; r += slice_rows) {
+      const int64_t n = std::min(slice_rows, tbl.fragments[f].num_tuples - r);
+      sl.push_back({f, r, n, chunks});
+      chunks += (n + chunk_rows - 1) / chunk_rows;
+      max_rows = std::max(max_rows, n);
+    }
+  run->written = run->scanned = 0;
+  const size_t ns = sl.size();
+  if (!ns || cap == 0) return B2Q_OK;
+  /* one device block: per-slice launch tables | status words | done, written, scanned, tickets[ns] | two staging sets */
+  const size_t tab_words = ns * nc + ns + 2 * ns + ns;
+  const size_t tab_bytes = DeviceBlock::pad(tab_words * 8), status_bytes = DeviceBlock::pad(static_cast<size_t>(chunks) * 8),
+               ctr_bytes = DeviceBlock::pad((3 + ns) * 8);
+  size_t stage_bytes = 0;
+  for (int c = 0; c < nc; ++c) stage_bytes += DeviceBlock::pad(static_cast<size_t>(max_rows) * q.prog.col_width[c] + 16);
+  int8_t* blk = nullptr;
+  CU(cudaMallocAsync(reinterpret_cast<void**>(&blk), tab_bytes + status_bytes + ctr_bytes + 2 * stage_bytes, st));
+  unsigned long long* status = reinterpret_cast<unsigned long long*>(blk + tab_bytes);
+  unsigned long long* counters = reinterpret_cast<unsigned long long*>(blk + tab_bytes + status_bytes);
+  int8_t* stage[2][B2Q_MAX_COLS];
+  for (int k = 0; k < 2; ++k) {
+    int8_t* at = blk + tab_bytes + status_bytes + ctr_bytes + k * stage_bytes;
+    for (int c = 0; c < nc; ++c) { stage[k][c] = at; at += DeviceBlock::pad(static_cast<size_t>(max_rows) * q.prog.col_width[c] + 16); }
+  }
+  std::vector<int64_t> host(tab_words);
+  int64_t* h_rows = host.data() + ns * nc;
+  int64_t* h_cs = h_rows + ns;
+  int64_t* h_base = h_cs + 2 * ns;
+  for (size_t i = 0; i < ns; ++i) {
+    for (int c = 0; c < nc; ++c) host[i * nc + c] = reinterpret_cast<int64_t>(stage[i & 1][c]);
+    h_rows[i] = sl[i].rows;
+    h_cs[2 * i] = 0;
+    h_cs[2 * i + 1] = (sl[i].rows + chunk_rows - 1) / chunk_rows;
+    h_base[i] = sl[i].row0;
+  }
+  const int64_t* d_tab = reinterpret_cast<const int64_t*>(blk);
+  size_t pin_cap = 0;
+  unsigned long long* h_ctr = reinterpret_cast<unsigned long long*>(pinned_cache().get(64, &pin_cap)); /* [0] done as last read, [1..3] final */
+  if (!h_ctr) { cudaFreeAsync(blk, st); return set_err(B2Q_ERR_INVALID_ARGUMENT, "out of (pinned) host memory"); }
+  h_ctr[0] = 0;
+  cudaStream_t copy_st = nullptr;
+  cudaEvent_t ready = nullptr, ev0 = nullptr, ev1 = nullptr, copied[2] = {}, scanned[2] = {};
+  bool busy[2] = {false, false};
+  cudaError_t e = cudaMemcpyAsync(blk, host.data(), tab_words * 8, cudaMemcpyHostToDevice, st);
+  if (e == cudaSuccess) e = cudaMemsetAsync(status, 0, status_bytes + ctr_bytes, st);
+  if (e == cudaSuccess) e = cudaStreamCreateWithFlags(&copy_st, cudaStreamNonBlocking);
+  for (cudaEvent_t* x : {&ready, &copied[0], &copied[1], &scanned[0], &scanned[1]})
+    if (e == cudaSuccess) e = cudaEventCreateWithFlags(x, cudaEventDisableTiming);
+  if (e == cudaSuccess) e = cudaEventCreate(&ev0);
+  if (e == cudaSuccess) e = cudaEventCreate(&ev1);
+  if (e == cudaSuccess) e = cudaEventRecord(ready, st); /* the block exists and is initialised before the copy stream writes into it */
+  if (e == cudaSuccess) e = cudaStreamWaitEvent(copy_st, ready, 0);
+  if (e == cudaSuccess) e = cudaEventRecord(ev0, st);
+  const int64_t row_size = q.plan.output_columnar ? 0 : q.plan.row_size;
+  for (size_t i = 0; i < ns && e == cudaSuccess; ++i) {
+    const int k = static_cast<int>(i & 1);
+    if (busy[k]) {
+      e = cudaEventSynchronize(scanned[k]); /* the scan that used this set, and the read of the done flag after it */
+      if (e != cudaSuccess || h_ctr[0]) break;
+      e = cudaStreamWaitEvent(copy_st, scanned[k], 0);
+    }
+    const Slice& x = sl[i];
+    for (int c = 0; c < nc && e == cudaSuccess; ++c) {
+      const int8_t* src = static_cast<const int8_t*>(tbl.fragments[x.frag].col_buffers[q.col_ids[c]]);
+      const size_t w = static_cast<size_t>(q.prog.col_width[c]);
+      e = cudaMemcpyAsync(stage[k][c], src + static_cast<size_t>(x.row0) * w, static_cast<size_t>(x.rows) * w, cudaMemcpyHostToDevice, copy_st);
+      *h2d_bytes += static_cast<double>(x.rows) * static_cast<double>(w);
+    }
+    if (e == cudaSuccess) e = cudaEventRecord(copied[k], copy_st);
+    if (e == cudaSuccess) e = cudaStreamWaitEvent(st, copied[k], 0);
+    if (e == cudaSuccess)
+      e = launch_project(q, reinterpret_cast<const int8_t* const*>(d_tab + i * nc), d_tab + ns * nc + i, d_tab + ns * nc + ns + 2 * i,
+                         d_tab + ns * nc + 3 * ns + i, 1, h_cs[2 * i + 1], x.chunk_base, d_out, row_size, cap, status, counters + 3 + i,
+                         counters, st);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(h_ctr, counters, 8, cudaMemcpyDeviceToHost, st);
+    if (e == cudaSuccess) e = cudaEventRecord(scanned[k], st);
+    busy[k] = true;
+  }
+  if (e == cudaSuccess) e = cudaEventRecord(ev1, st);
+  if (e == cudaSuccess) e = cudaMemcpyAsync(h_ctr + 1, counters, 3 * 8, cudaMemcpyDeviceToHost, st);
+  cudaFreeAsync(blk, st);
+  if (e == cudaSuccess) e = cudaStreamSynchronize(st);
+  if (copy_st) { cudaStreamSynchronize(copy_st); cudaStreamDestroy(copy_st); }
+  float ms = 0;
+  if (e == cudaSuccess && cudaEventElapsedTime(&ms, ev0, ev1) == cudaSuccess) run->kernel_ms = ms;
+  for (cudaEvent_t x : {ready, ev0, ev1, copied[0], copied[1], scanned[0], scanned[1]}) if (x) cudaEventDestroy(x);
+  if (e == cudaSuccess) { run->written = static_cast<int64_t>(h_ctr[2]); run->scanned = static_cast<int64_t>(h_ctr[3]); }
+  pinned_cache().put(reinterpret_cast<int8_t*>(h_ctr), pin_cap);
+  if (e != cudaSuccess) { cudaGetLastError(); return set_err(e == cudaErrorMemoryAllocation ? B2Q_ERR_OUT_OF_GPU_MEM : B2Q_ERR_CUDA, std::string("projection (host table): ") + cudaGetErrorString(e)); }
+  return B2Q_OK;
+}
+
+/* the layout of a projection buffer for `n` entries: row-wise the prefix of a longer buffer, columnar every column moves */
+static void projection_relayout(B2QQuery& q, int64_t n) {
+  relayout_entries(q.plan, n);
+  for (int s = 0; s < q.proj.n; ++s) q.proj.cols[s].out_off = q.plan.slot_offset[s];
+}
+
+/* a columnar buffer written for `cap` entries holding `n`: the same columns at stride n, padding zeroed (the bytes the
+ * reference's descriptor would have for an n-entry buffer) */
+static cudaError_t projection_compact(const B2QPlan& at_cap, const B2QPlan& at_n, const int8_t* d_in, int8_t* d_out, cudaStream_t st) {
+  const int64_t n = at_n.entry_count;
+  auto one = [&](int64_t in_off, int64_t out_off, int w) -> cudaError_t {
+    const int64_t bytes = w * n, padded = (bytes + 7) & ~int64_t(7);
+    cudaError_t e = cudaSuccess;
+    if (d_in + in_off != d_out + out_off && bytes) e = cudaMemcpyAsync(d_out + out_off, d_in + in_off, bytes, cudaMemcpyDeviceToDevice, st);
+    if (e == cudaSuccess && padded > bytes) e = cudaMemsetAsync(d_out + out_off + bytes, 0, padded - bytes, st);
+    return e;
+  };
+  cudaError_t e = one(0, 0, 8);
+  for (int s = 0; s < at_n.num_slots && e == cudaSuccess; ++s) e = one(at_cap.slot_offset[s], at_n.slot_offset[s], at_n.slot_padded_width[s]);
+  return e;
+}
+
+/* COUNT(*) over the quals of a projection unit: the pre-flight that sizes a projection without a scan limit */
+static int32_t projection_count(const B2QTableInfo* tbl, const B2QExecUnit* u, const B2QCompilationOptions* co,
+                                const B2QExecutionOptions* eo, cudaStream_t st, int64_t* count, double* h2d_bytes) {
+  std::vector<B2QExpr> exprs(u->exprs, u->exprs + u->num_exprs);
+  B2QExpr cnt;
+  memset(&cnt, 0, sizeof(cnt));
+  cnt.kind = B2Q_EXPR_AGG;
+  cnt.ti.type = B2Q_kBIGINT;
+  cnt.op = B2Q_kCOUNT;
+  cnt.left = cnt.right = -1;
+  exprs.push_back(cnt);
+  const int32_t target = static_cast<int32_t>(exprs.size()) - 1;
+  B2QExecUnit cu = *u;
+  cu.exprs = exprs.data();
+  cu.num_exprs = static_cast<int32_t>(exprs.size());
+  cu.target_exprs = &target;
+  cu.num_target_exprs = 1;
+  cu.num_order_entries = 0;
+  cu.has_limit = 0;
+  cu.limit = cu.offset = 0;
+  cu.scan_limit = 0;
+  B2QExecutionOptions ceo = *eo;
+  ceo.bigint_count = 1;
+  ceo.result_on_device = 0;
+  ceo.output_columnar_hint = 0;
+  ceo.force_kernel = 0;
+  B2QPartial* p = nullptr;
+  int32_t rc = execute_partial_attempt(nullptr, tbl, &cu, co, &ceo, 0, st, false, false, &p);
+  if (rc != B2Q_OK) return rc;
+  std::unique_ptr<B2QPartial> own(p);
+  B2QResultSet* crs = nullptr;
+  rc = finalize_impl(p, st, &crs);
+  if (rc != B2Q_OK) return rc;
+  std::unique_ptr<B2QResultSet> rs(crs);
+  B2QTargetValue v;
+  b2q_read_target(rs->q.plan, rs->buf, 0, 0, false, &v);
+  *count = v.is_null ? 0 : v.ival;
+  *h2d_bytes += rs->h2d_bytes;
+  return B2Q_OK;
+}
+
+/* Executor::executeWorkUnit for a projection unit (QueryDescriptionType::Projection, is_agg = false) */
+static int32_t execute_projection(const B2QTableInfo* tbl, const B2QExecUnit* u, const B2QCompilationOptions* co,
+                                  const B2QExecutionOptions* eo, B2QResultSet** out) {
+  if (!tbl || !u || !co || !eo || !out) return set_err(B2Q_ERR_INVALID_ARGUMENT, "null argument");
+  if (co->device_type != B2Q_DEVICE_GPU) return set_err(B2Q_ERR_UNSUPPORTED, "device_type must be GPU: this path has no CPU execution");
+  std::unique_ptr<B2QResultSet> rs(new B2QResultSet());
+  std::string err;
+  int32_t rc = make_query(u, tbl, eo, 0, false, !co->ignore_deleted_column, &rs->q, &err);
+  if (rc != B2Q_OK) return set_err(rc, err);
+  if (!have_device()) return set_err(B2Q_ERR_NO_DEVICE, "no CUDA device visible; this path has no CPU fallback");
+  if (tbl->memory_level != B2Q_GPU_LEVEL && tbl->memory_level != B2Q_CPU_LEVEL)
+    return set_err(B2Q_ERR_INVALID_ARGUMENT, "memory_level must be B2Q_CPU_LEVEL or B2Q_GPU_LEVEL");
+  if (eo->device_ordinal >= 0) CU(cudaSetDevice(eo->device_ordinal));
+  int device = 0;
+  CU(cudaGetDevice(&device));
+  configure_pool_once(device);
+  cudaStream_t st = nullptr;
+  const bool filter_deleted = !co->ignore_deleted_column;
+  B2QQuery& q = rs->q;
+  /* fragments in fragment-id order (the order resultsUnion gives per-fragment results), skipped ones left out */
+  std::vector<int> frags;
+  for (int f = 0; f < tbl->num_fragments; ++f) frags.push_back(f);
+  std::stable_sort(frags.begin(), frags.end(), [&](int a, int b) { return tbl->fragments[a].fragment_id < tbl->fragments[b].fragment_id; });
+  std::vector<int> scanned_frags;
+  std::vector<const int8_t*> cols;
+  std::vector<int64_t> rows;
+  int64_t tuples = 0;
+  for (int f : frags) {
+    if (skip_fragment(*u, *tbl, tbl->fragments[f], filter_deleted)) { rs->frags_skipped += 1; continue; }
+    rs->frags_scanned += 1;
+    scanned_frags.push_back(f);
+    rows.push_back(tbl->fragments[f].num_tuples);
+    tuples += tbl->fragments[f].num_tuples;
+    for (int c = 0; c < q.prog.n_cols; ++c) {
+      const void* ptr = tbl->fragments[f].col_buffers[q.col_ids[c]];
+      if (!ptr) return set_err(B2Q_ERR_INVALID_ARGUMENT, "referenced column has a NULL buffer");
+      cols.push_back(static_cast<const int8_t*>(ptr));
+    }
+  }
+  /* capacity: LIMIT 0 is an empty result (RelSort::isEmptyResult); else the scan limit, never more than the rows scanned; else
+   * the exact number of passing rows (the pre-flight: one more scan and one more host wait) */
+  int64_t cap = std::min<int64_t>(u->scan_limit, tuples);
+  if (q.has_limit && q.limit == 0) {
+    cap = 0;
+  } else if (u->scan_limit == 0) {
+    rc = projection_count(tbl, u, co, eo, st, &cap, &rs->h2d_bytes);
+    if (rc != B2Q_OK) return rc;
+    rs->launches += 2;
+  }
+  projection_relayout(q, cap);
+  const B2QPlan at_cap = q.plan;
+  int8_t* d_out = nullptr;
+  CU(cudaMallocAsync(reinterpret_cast<void**>(&d_out), std::max<int64_t>(at_cap.buffer_size, 8), st));
+  ProjectRun run;
+  if (tbl->memory_level == B2Q_CPU_LEVEL) rc = project_scan_host(q, *tbl, scanned_frags, d_out, cap, st, &run, &rs->h2d_bytes);
+  else rc = project_scan(q, static_cast<int>(rows.size()), cols, rows, d_out, cap, st, &run);
+  if (rc != B2Q_OK) { cudaFreeAsync(d_out, st); return rc; }
+  rs->launches += rows.empty() ? 0 : 1;
+  rs->scan_ms = run.kernel_ms;
+  rs->rows_scanned = run.scanned;
+  /* the result holds exactly the rows written (compactProjectionBuffersGpu, QueryMemoryInitializer.cpp:1408-1431) */
+  projection_relayout(q, run.written);
+  int8_t* d_res = d_out;
+  cudaError_t e = cudaSuccess;
+  if (q.plan.output_columnar) {
+    if (run.written < cap) {
+      d_res = nullptr;
+      e = cudaMallocAsync(reinterpret_cast<void**>(&d_res), std::max<int64_t>(q.plan.buffer_size, 8), st);
+      if (e == cudaSuccess) e = projection_compact(at_cap, q.plan, d_out, d_res, st);
+      cudaFreeAsync(d_out, st);
+    } else {
+      e = projection_compact(at_cap, q.plan, d_out, d_out, st); /* zero the column padding only */
+    }
+  }
+  if (e != cudaSuccess) { if (d_res) cudaFreeAsync(d_res, st); cudaGetLastError(); return set_err(B2Q_ERR_CUDA, std::string("projection compaction: ") + cudaGetErrorString(e)); }
+  const bool want_sort = q.n_order > 0 || q.has_limit || q.offset > 0;
+  if (q.plan.buffer_size && want_sort) {
+    rc = sort_keep_rows(rs.get(), d_res, eo->result_on_device != 0, device, st);
+    if (rc != B2Q_OK) return rc;
+    *out = rs.release();
+    return B2Q_OK;
+  }
+  rs->buf_size = static_cast<size_t>(q.plan.buffer_size);
+  if (!rs->buf_size) {
+    cudaFreeAsync(d_res, st);
+  } else if (eo->result_on_device) {
+    rs->d_buf = d_res;
+    rs->device = device;
+  } else {
+    rs->buf = pinned_cache().get(rs->buf_size, &rs->buf_cap);
+    if (!rs->buf) { cudaFreeAsync(d_res, st); return set_err(B2Q_ERR_INVALID_ARGUMENT, "out of (pinned) host memory for the result buffer"); }
+    e = cudaMemcpyAsync(rs->buf, d_res, rs->buf_size, cudaMemcpyDeviceToHost, st);
+    rs->d2h_bytes = static_cast<int64_t>(rs->buf_size);
+    cudaFreeAsync(d_res, st);
+  }
+  if (e == cudaSuccess) e = cudaStreamSynchronize(st);
+  if (e != cudaSuccess) { cudaGetLastError(); return set_err(B2Q_ERR_CUDA, std::string("projection result: ") + cudaGetErrorString(e)); }
+  *out = rs.release();
+  return B2Q_OK;
+}
+
+static bool is_projection_unit(const B2QExecUnit* u) {
+  if (!u || u->has_estimator || u->num_groupby_exprs != 0 || u->num_target_exprs <= 0 || !u->target_exprs || !u->exprs) return false;
+  for (int i = 0; i < u->num_target_exprs; ++i) {
+    const int t = u->target_exprs[i];
+    if (t < 0 || t >= u->num_exprs || u->exprs[t].kind != B2Q_EXPR_COLUMN_VAR) return false;
+  }
+  return true;
+}
+
 /* The entry points select eo->device_ordinal / the partial's / the communicator's device; the caller gets its own current
  * device back when they return (the work they enqueued stays bound to its stream). */
 struct CallerDevice {
@@ -1307,6 +1657,7 @@ int32_t b2q_execute_work_unit(size_t* guess, int32_t is_agg, const B2QTableInfo*
                               B2QResultSet** out) {
   (void)is_agg;
   CallerDevice restore;
+  if (is_projection_unit(u) && !u->num_join_quals) return execute_projection(tbl, u, co, eo, out);
   g_trace.begin();
   for (int attempt = 0; attempt < 2; ++attempt) {
     B2QPartial* p = nullptr;
@@ -1354,6 +1705,30 @@ int32_t b2q_launch(const B2QQuery* query, const B2QParams* prm, void* stream) {
     return set_err(B2Q_ERR_INVALID_ARGUMENT, "missing kernel parameter");
   if (prm->num_tables && *prm->num_tables != (has_join ? 2u : 1u)) return set_err(B2Q_ERR_UNSUPPORTED, "number of input tables does not match the plan");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
+  if (query->plan.query_desc_type == B2Q_Projection) { /* rows at TOTAL_MATCHED++ up to MAX_MATCHED, in (fragment, row) order */
+    B2QQuery q = *query;
+    const int nf = static_cast<int>(*prm->num_fragments);
+    std::vector<const int8_t*> cols(static_cast<size_t>(nf) * q.prog.n_cols);
+    std::vector<int64_t> rows(nf);
+    for (int f = 0; f < nf; ++f) {
+      rows[f] = prm->num_rows[f];
+      for (int c = 0; c < q.prog.n_cols; ++c) cols[static_cast<size_t>(f) * q.prog.n_cols + c] = prm->col_buffers[f][q.col_ids[c]];
+    }
+    const int64_t cap = prm->max_matched ? *prm->max_matched : q.plan.entry_count;
+    if (cap < 0) return set_err(B2Q_ERR_INVALID_ARGUMENT, "MAX_MATCHED is negative");
+    projection_relayout(q, cap);
+    int64_t* d_out = nullptr;
+    CU(cudaMemcpyAsync(&d_out, prm->group_by_buffers, sizeof(int64_t*), cudaMemcpyDefault, st));
+    CU(cudaStreamSynchronize(st));
+    ProjectRun run;
+    const int32_t rc = project_scan(q, nf, cols, rows, reinterpret_cast<int8_t*>(d_out), cap, st, &run);
+    if (rc != B2Q_OK) return rc;
+    const int32_t matched = static_cast<int32_t>(std::min<int64_t>(run.written, INT32_MAX));
+    if (prm->total_matched) CU(cudaMemcpy(prm->total_matched, &matched, sizeof(int32_t), cudaMemcpyDefault));
+    const int32_t ok = 0;
+    if (prm->error_codes) CU(cudaMemcpy(prm->error_codes, &ok, sizeof(int32_t), cudaMemcpyDefault));
+    return B2Q_OK;
+  }
   B2QPartial p;
   p.q = *query;
   if (prm->init_agg_value) {
@@ -1612,6 +1987,7 @@ int64_t b2q_rs_stat(const B2QResultSet* rs, int32_t which) {
     case B2Q_STAT_HOST_STREAM_US: return static_cast<int64_t>(rs->host_stream_us);
     case B2Q_STAT_HOST_TEARDOWN_US: return static_cast<int64_t>(rs->host_teardown_us);
     case B2Q_STAT_RESULT_D2H_BYTES: return rs->d2h_bytes;
+    case B2Q_STAT_ROWS_SCANNED: return rs->rows_scanned;
     default: return -1;
   }
 }

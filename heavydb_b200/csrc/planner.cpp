@@ -134,6 +134,10 @@ class Planner {
       choose_kernel(q);
       return;
     }
+    if (is_projection()) {
+      plan_projection(q);
+      return;
+    }
     build_targets();
     for (int i = 0; i < u_.num_order_entries; ++i) { /* the device sort orders 8-byte images; float slots would need their own */
       const TargetDesc& d = targets_[u_.order_entries[i].tle_no - 1];
@@ -205,6 +209,90 @@ class Planner {
     p.join_entry_count = entries;
     p.join_outer_col = join_outer_col_;
     p.join_inner_col = join_inner_col_;
+  }
+
+  /* QueryDescriptionType::Projection: groupby_exprs == {nullptr} and every target a plain ColumnVar */
+  bool is_projection() const {
+    if (u_.has_estimator || u_.num_groupby_exprs != 0) return false;
+    for (int i = 0; i < u_.num_target_exprs; ++i)
+      if (ex(u_.target_exprs[i]).kind != B2Q_EXPR_COLUMN_VAR) return false;
+    return true;
+  }
+
+  /* QueryMemoryDescriptor::init, Projection branch (QueryMemoryDescriptor.cpp:394-418) without lazy fetch
+   * (target_groupby_indices empty: the boundary does not hand the caller's chunks to the result set, so every target is
+   * materialised).  entry_count = scan_limit, or every row of the table when there is none (the executor then sizes the
+   * allocation from a COUNT(*) pre-flight).  Slots: ColSlotContext's logical sizes; row-wise every slot is padded to 8
+   * (setAllUnsetSlotsPaddedSize(8), :507), columnar they stay logical-sized (isLogicalSizedColumnsAllowed, :540-546).
+   * Layout: row-wise [int64 offset in fragment][slots] (get_scan_output_slot, GroupByRuntime.cpp:242-254), columnar
+   * [int64 offsets column][slot columns] (get_columnar_scan_output_offset, :256-266). */
+  void plan_projection(B2QQuery& q) {
+    if (join_) reject(B2Q_ERR_UNSUPPORTED, "a projection with a join level is outside this path");
+    if (u_.scan_limit < 0) reject(B2Q_ERR_INVALID_ARGUMENT, "negative scan_limit");
+    for (int i = 0; i < u_.num_target_exprs; ++i) {
+      const B2QExpr& e = ex(u_.target_exprs[i]);
+      const SqlType ct = col_type(e.col_id);
+      if (t_.col_types[e.col_id].type == B2Q_kBOOLEAN) reject(B2Q_ERR_UNSUPPORTED, "projecting the deleted-rows column is outside this path");
+      if (from_abi(e.ti).size() != ct.size()) reject(B2Q_ERR_INVALID_ARGUMENT, "ColumnVar type does not match the table");
+      TargetDesc d;
+      d.sql_type = from_abi(e.ti);
+      d.arg_col = e.col_id;
+      d.first_slot = i;
+      targets_.push_back(d);
+    }
+    for (int i = 0; i < u_.num_order_entries; ++i) {
+      const SqlType& t = targets_[u_.order_entries[i].tle_no - 1].sql_type;
+      if (t.is_float()) reject(B2Q_ERR_UNSUPPORTED, "ORDER BY a FLOAT target is outside this path");
+      if (t.is_string()) reject(B2Q_ERR_UNSUPPORTED, "ORDER BY a dictionary-encoded string needs the dictionary");
+    }
+    B2QPlan& p = q.plan;
+    p.query_desc_type = B2Q_Projection;
+    p.key_col_id = -1;
+    p.idx_target_as_key = -1;
+    p.effective_key_width = 8;
+    p.num_group_cols = 0;
+    int64_t tuples = 0;
+    for (int f = 0; f < t_.num_fragments; ++f) tuples += t_.fragments[f].num_tuples;
+    p.entry_count = u_.scan_limit ? u_.scan_limit : tuples;
+    p.num_targets = p.num_slots = static_cast<int32_t>(targets_.size());
+    p.output_columnar = eo_.output_columnar_hint ? 1 : 0;
+    int64_t off = p.output_columnar ? align8(8 * p.entry_count) : 8, cols = 0;
+    for (int s = 0; s < p.num_slots; ++s) {
+      const int8_t logical = static_cast<int8_t>(targets_[s].sql_type.size());
+      p.slot_logical_width[s] = logical;
+      p.slot_padded_width[s] = p.output_columnar ? logical : 8;
+      p.slot_offset[s] = off;
+      off += p.output_columnar ? align8(logical * p.entry_count) : 8;
+      cols += p.slot_padded_width[s];
+      p.init_vals[s] = 0;
+    }
+    p.row_size = p.output_columnar ? align8(cols) : off;
+    p.buffer_size = p.output_columnar ? off : p.row_size * p.entry_count;
+    publish_targets(p);
+    lower_filter(q);
+    DevProject& P = q.proj;
+    P.n = p.num_targets;
+    P.scan_limit = u_.scan_limit;
+    for (int s = 0; s < P.n; ++s) {
+      const int c = targets_[s].arg_col;
+      const SqlType ct = col_type(c);
+      DevProjCol& pc = P.cols[s];
+      pc.col = launch_col(q, c);
+      pc.width = static_cast<int8_t>(phys_width_code(c));
+      pc.kind = ct.is_float() ? PROJ_F32 : ct.is_fp() ? PROJ_F64 : PROJ_INT;
+      pc.days = is_days(c) ? 1 : 0;
+      pc.null_phys = ct.is_fp() ? 0 : phys_int_null(c);
+      pc.null_logical = ct.is_fp() ? 0 : ct.int_null();
+      pc.translate_null = !ct.is_fp() && !ct.notnull && (pc.days || pc.null_phys != pc.null_logical);
+      pc.out_w = p.slot_padded_width[s];
+      pc.out_off = p.slot_offset[s];
+    }
+    q.n_order = u_.num_order_entries;
+    for (int i = 0; i < u_.num_order_entries; ++i) q.order[i] = u_.order_entries[i];
+    q.has_limit = u_.has_limit ? 1 : 0;
+    q.limit = u_.limit;
+    q.offset = u_.offset;
+    q.total_tuples = tuples;
   }
 
   /* QueryDescriptionType::Estimator (QueryMemoryDescriptor::init :270-300): entry_count 1, the output is the
@@ -1281,19 +1369,9 @@ class Planner {
     return a;
   }
 
-  void lower(B2QQuery& q) {
-    B2QPlan& p = q.plan;
+  /* the quals (and the deleted-rows test) as the device program's filter */
+  void lower_filter(B2QQuery& q) {
     DevProgram& g = q.prog;
-    q.bigint_count = eo_.bigint_count;
-    if (join_) { /* probe parameters: hash_join_idx[_nullable](buff, key, min, max[, null]) (GroupByRuntime.cpp:283-311) */
-      g.join.fk_col = launch_col(q, join_outer_col_);
-      g.join.fk_width = static_cast<int8_t>(phys_width_code(join_outer_col_));
-      g.join.min_key = p.join_min_key;
-      g.join.entry_count = p.join_entry_count;
-      g.join.nullable = !col_type(join_outer_col_).notnull;
-      g.join.null_val = phys_int_null(join_outer_col_);
-      g.join.left = join_left_ ? 1 : 0;
-    }
     /* filter: all simple_quals and quals AND-ed */
     int n_quals = 0, max_depth = 0;
     auto add_qual = [&](int idx) {
@@ -1346,6 +1424,23 @@ class Planner {
     g.est_selectivity = static_cast<float>(estimate_selectivity(g.filter));
     g.eager_key = g.est_selectivity >= 0.10f;
     g.eager_args = g.est_selectivity >= 0.25f;
+  }
+
+  void lower(B2QQuery& q) {
+    B2QPlan& p = q.plan;
+    DevProgram& g = q.prog;
+    q.bigint_count = eo_.bigint_count;
+    if (join_) { /* probe parameters: hash_join_idx[_nullable](buff, key, min, max[, null]) (GroupByRuntime.cpp:283-311) */
+      g.join.fk_col = launch_col(q, join_outer_col_);
+      g.join.fk_width = static_cast<int8_t>(phys_width_code(join_outer_col_));
+      g.join.min_key = p.join_min_key;
+      g.join.entry_count = p.join_entry_count;
+      g.join.nullable = !col_type(join_outer_col_).notnull;
+      g.join.null_val = phys_int_null(join_outer_col_);
+      g.join.left = join_left_ ? 1 : 0;
+    }
+    lower_filter(q);
+
 
     if (u_.has_estimator) { /* the tuple rides in keys[]; ONE accumulator: the bitmap (see ACC_NDV) */
       g.n_keys = static_cast<int32_t>(estimator_cols_.size());

@@ -40,6 +40,8 @@ __device__ __forceinline__ const int8_t* slot_addr(const DevSortLayout& L, const
 }
 __device__ __forceinline__ int64_t read_slot(const DevSortLayout& L, const int8_t* buf, int64_t e, int64_t off, int w) {
   const int8_t* p = slot_addr(L, buf, e, off, w);
+  if (w == 1) return *p; /* logical-sized columns of a columnar projection */
+  if (w == 2) return *reinterpret_cast<const int16_t*>(p);
   return w == 4 ? (int64_t) * reinterpret_cast<const int32_t*>(p) : *reinterpret_cast<const int64_t*>(p);
 }
 /* ResultSetStorage::isEmptyEntry / isEmptyEntryColumnar (ResultSetIteration.cpp:2457-2545) */
@@ -365,11 +367,16 @@ __global__ void b2q_k_sort_gather(const DevSortLayout Lin, const int8_t* __restr
   for (int64_t r = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; r < n_out; r += stride) {
     const int64_t e = perm[first + r];
     for (int c = 0; c < G.n; ++c) {
-      if (G.width[c] == 4) reinterpret_cast<int32_t*>(out + G.out_off[c])[r] = reinterpret_cast<const int32_t*>(in + G.in_off[c])[e];
-      else reinterpret_cast<int64_t*>(out + G.out_off[c])[r] = reinterpret_cast<const int64_t*>(in + G.in_off[c])[e];
+      switch (G.width[c]) {
+        case 1: (out + G.out_off[c])[r] = (in + G.in_off[c])[e]; break;
+        case 2: reinterpret_cast<int16_t*>(out + G.out_off[c])[r] = reinterpret_cast<const int16_t*>(in + G.in_off[c])[e]; break;
+        case 4: reinterpret_cast<int32_t*>(out + G.out_off[c])[r] = reinterpret_cast<const int32_t*>(in + G.in_off[c])[e]; break;
+        default: reinterpret_cast<int64_t*>(out + G.out_off[c])[r] = reinterpret_cast<const int64_t*>(in + G.in_off[c])[e];
+      }
     }
-    if (r == n_out - 1 && (n_out & 1)) /* column padding of 4-byte columns with an odd entry count (recycled buffer) */
-      for (int c = 0; c < G.n; ++c) if (G.width[c] == 4) reinterpret_cast<int32_t*>(out + G.out_off[c])[n_out] = 0;
+    if (r == n_out - 1) /* column padding of narrow columns up to 8 bytes (recycled buffer) */
+      for (int c = 0; c < G.n; ++c)
+        for (int64_t b = n_out * G.width[c]; b & 7; ++b) (out + G.out_off[c])[b] = 0;
   }
 }
 

@@ -283,7 +283,8 @@ class ResultSet:
                 "kernel_launches": L.b2q_rs_stat(self._h, 2), "h2d_bytes": L.b2q_rs_stat(self._h, 3),
                 "sort_us": L.b2q_rs_stat(self._h, 4), "host_setup_us": L.b2q_rs_stat(self._h, 5),
                 "host_stream_us": L.b2q_rs_stat(self._h, 6), "host_teardown_us": L.b2q_rs_stat(self._h, 7),
-                "result_d2h_bytes": L.b2q_rs_stat(self._h, abi.STAT_RESULT_D2H_BYTES)}
+                "result_d2h_bytes": L.b2q_rs_stat(self._h, abi.STAT_RESULT_D2H_BYTES),
+                "rows_scanned": L.b2q_rs_stat(self._h, abi.STAT_ROWS_SCANNED)}
 
     def columnarResults(self, num_threads: int = 8, with_scale: bool = False):
         """ColumnarResults(rows, num_columns, target_types) (QueryEngine/ColumnarResults.cpp:256-392): one numpy array per

@@ -302,4 +302,9 @@ def parse(sql: str, table: abi.Table, names: List[str], bigint_count: bool = Fal
         raise ValueError(f"trailing tokens: {p.t[p.i:]}")
     for t in targets:
         p.b.target(t)
+    # get_scan_limit (RelAlgExecutor.cpp:3442-3449, :3630-3632): LIMIT without ORDER BY over a non-aggregate source scans at
+    # most limit + offset rows; aggregate units keep scan_limit 0
+    aggregate = p.b.groupby or any(p.b.nodes[t].kind == abi.EXPR_AGG for t in targets)
+    if not aggregate and p.b.estimator_kind == 0 and not p.b.order and p.b.limit is not None:
+        p.b.scan_limit = p.b.limit + p.b.offset
     return p.b.build()

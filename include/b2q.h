@@ -37,7 +37,7 @@
 extern "C" {
 #endif
 
-#define B2Q_ABI_VERSION 6 /* 2: sort_info, join level, rte_idx, columnar, dictionary / time types, B2QPlan join fields;
+#define B2Q_ABI_VERSION 7 /* 2: sort_info, join level, rte_idx, columnar, dictionary / time types, B2QPlan join fields;
                             3: DATE_IN_DAYS chunks (negative col_encoded_sizes), column-vs-column quals, 16 filter leaves,
                                operands-before-node rule, b2q_columnar_results_*, host-phase stats;
                             4: DECIMAL / NUMERIC columns (B2QTypeInfo.scale), decimal_to_double of b2q_rs_get_next_row;
@@ -46,7 +46,9 @@ extern "C" {
                                (B2QPlan.count_distinct_*);
                             6: B2QExecutionOptions.result_on_device (was pad_), B2QDeviceColumns / b2q_rs_device_columns /
                                b2q_device_columns_* (ColumnarResults in device memory, Arrow C Device export, b2q_arrow.h),
-                               B2Q_STAT_RESULT_D2H_BYTES */
+                               B2Q_STAT_RESULT_D2H_BYTES;
+                            7: projection units (B2Q_Projection: column targets, no GROUP BY, B2QExecUnit.scan_limit),
+                               B2Q_STAT_ROWS_SCANNED, TOTAL_MATCHED / MAX_MATCHED of b2q_launch */
 
 /* ---- SQLTypes subset (Shared/sqltypes.h:65-99) -------------------------------------------------------- */
 enum {
@@ -167,6 +169,10 @@ typedef struct B2QExecUnit {
   int32_t num_groupby_exprs;
   const int32_t* target_exprs; /* expr indices */
   int32_t num_target_exprs;
+  /* Projection units (no groupby_exprs, every target a ColumnVar, no aggregate): the output holds at most scan_limit rows,
+   * the first passing rows in (fragment, row) order — what RelAlgExecutor sets for LIMIT without ORDER BY (limit + offset,
+   * get_scan_limit, RelAlgExecutor.cpp:3442-3449).  0 = no limit: the library counts the passing rows first (the non-grouped
+   * COUNT(*) scan over the same quals) and sizes the output from that count. */
   int64_t scan_limit;
   /* join_quals (JoinQualsPerNestingLevel, RelAlgExecutionUnit.h:166-216): at most ONE nesting level, INNER or LEFT,
    * whose only qual is `ColumnVar(rte 0) = ColumnVar(rte 1)` over integer columns and for which the reference would
@@ -351,7 +357,7 @@ typedef struct B2QPlan {
 /* The 15-slot kernel parameter block of the reference's JIT entry (enums.h:64-79), device pointers. */
 typedef struct B2QParams {
   int32_t* error_codes;            /* ERROR_CODE      */
-  int32_t* total_matched;          /* TOTAL_MATCHED   */
+  int32_t* total_matched;          /* TOTAL_MATCHED   projection: receives the rows written (may be NULL) */
   int64_t** group_by_buffers;      /* GROUPBY_BUF     — [0] = the output buffer in reference layout */
   const uint32_t* num_fragments;   /* NUM_FRAGMENTS   (host pointer, read on the host)   */
   const uint32_t* num_tables;      /* NUM_TABLES      (must point at 1) */
@@ -361,7 +367,8 @@ typedef struct B2QParams {
   const int64_t* num_rows;         /* NUM_ROWS        host array [frag] */
   const uint64_t* frag_row_offsets;/* FRAG_ROW_OFFSETS (unused) */
   const int32_t* frag_ids;         /* FRAG_IDS        (unused) */
-  const int32_t* max_matched;      /* MAX_MATCHED     (unused) */
+  const int32_t* max_matched;      /* MAX_MATCHED     (host pointer; projection: the output's capacity in rows, NULL = the plan's
+                                      entry_count; unused otherwise) */
   const int64_t* init_agg_value;   /* INIT_AGG_VALS   host array [num_slots]; NULL = plan->init_vals */
   const int64_t* join_hash_tables; /* JOIN_HASH_TABLES NULL, or [0] = device address of the int32 one-to-one table
                                       (what HashJoin::getJoinHashBuffer returns) when the plan has a join level */
@@ -513,7 +520,9 @@ enum { B2Q_STAT_FRAGMENTS_SCANNED = 0, B2Q_STAT_FRAGMENTS_SKIPPED = 1 /* Executo
        /* host wall-clock of the CPU_LEVEL streaming scan: staging setup, copy+scan pipeline, teardown */
        B2Q_STAT_HOST_SETUP_US = 5, B2Q_STAT_HOST_STREAM_US = 6, B2Q_STAT_HOST_TEARDOWN_US = 7,
        B2Q_STAT_RESULT_D2H_BYTES = 8 /* result-storage bytes copied device -> host so far (0 for a result_on_device set no host
-                                        accessor has read yet) */ };
+                                        accessor has read yet) */,
+       B2Q_STAT_ROWS_SCANNED = 9 /* projection: rows of the chunks the projection kernel loaded (a scan limit stops it early);
+                                    0 for every other query */ };
 int64_t b2q_rs_stat(const B2QResultSet* rs, int32_t which);
 void b2q_rs_free(B2QResultSet* rs);
 /* ResultSet(targets, device_type, query_mem_desc, ...) + allocateStorage(buffer) (ResultSet.h:183-217): a result set over a
