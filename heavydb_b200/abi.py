@@ -529,7 +529,7 @@ class BuiltUnit:
 
 
 def chunk_stats(arr: np.ndarray, sql_type: int, notnull: bool, null=None) -> ChunkStats:
-    """ChunkMetadata::chunkStats as the reference's encoders maintain them: min/max over NON-NULL values,
+    """ChunkMetadata::chunkStats as the reference's encoders maintain them: min/max over NON-NULL values (NaN ignored),
     has_nulls when a NULL sentinel is present (DataMgr/Encoder.h; FixedLengthEncoder::updateStats)."""
     st = ChunkStats()
     null = NULL_OF[sql_type] if null is None else null
@@ -545,6 +545,7 @@ def chunk_stats(arr: np.ndarray, sql_type: int, notnull: bool, null=None) -> Chu
         vals = arr[mask]
         st.has_nulls = int(vals.size != arr.size)
     if sql_type in (kDOUBLE, kFLOAT):
+        vals = vals[~np.isnan(vals)]   # std::min(dataMin, NaN) keeps dataMin: the encoder never records a NaN
         if vals.size:
             st.fp_min, st.fp_max = float(vals.min()), float(vals.max())
         else:

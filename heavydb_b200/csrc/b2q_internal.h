@@ -195,7 +195,9 @@ struct DevSlot {
   int8_t scale_day;    /* MIN / MAX over a days-encoded DATE chunk: the accumulator holds days, the slot seconds */
   int8_t as_float;     /* FLOAT argument (takes_float_argument, TargetInfo.h:106-110): the accumulator is a double; the slot gets
                           its float image in the low 4 bytes, the high 4 bytes keep the init pattern's (agg_*_float write 32 bits) */
-  int8_t pad_[3];
+  int8_t clamp_init;   /* SLOT_VALUE_ORD over a NOT NULL argument: the reference starts from +-DBL_MAX (+-FLT_MAX), which neither
+                          +-inf nor a NaN can beat; the accumulator is clamped to that init value at materialise (b2q_clamp_ord) */
+  int8_t pad_[2];
   int32_t bm_words;    /* SLOT_BITCOUNT: 32-bit words per entry */
   int32_t pad2_;
 };
@@ -233,6 +235,26 @@ struct DevLayout {
 #endif
 B2Q_HD int64_t b2q_f64_to_ord(int64_t bits) { return bits ^ ((bits >> 63) & B2Q_I64_MAX); }
 B2Q_HD int64_t b2q_ord_to_f64(int64_t ord) { return ord ^ ((ord >> 63) & B2Q_I64_MAX); }
+/* MIN / MAX of doubles: std::min(old, NaN) keeps old, so a NaN never beats a number (RuntimeFunctions.cpp:1458-1468), yet a
+ * group whose values are ALL NaN does not end "empty": the nullable form assigns its first value and ends at NaN
+ * (DEF_SKIP_AGG, :1558-1569), the NOT NULL form keeps its init value (std::min(DBL_MAX, NaN)).  So a NaN enters the
+ * order-preserving accumulator as the image next to the identity (a NaN bit pattern itself): it loses to every number and is
+ * still told apart from "no value seen" at materialise. */
+B2Q_HD bool b2q_bits_is_nan(int64_t bits) { return (bits & B2Q_I64_MAX) > 0x7FF0000000000000LL; }
+B2Q_HD int64_t b2q_f64_min_ord(int64_t bits) { return b2q_bits_is_nan(bits) ? B2Q_I64_MAX - 1 : b2q_f64_to_ord(bits); }
+B2Q_HD int64_t b2q_f64_max_ord(int64_t bits) { return b2q_bits_is_nan(bits) ? B2Q_I64_MIN + 1 : b2q_f64_to_ord(bits); }
+/* NOT NULL MIN / MAX of a double start from the init value DBL_MAX / -DBL_MAX (FLT_MAX / -FLT_MAX for a FLOAT argument) instead
+ * of an identity: agg_min_double(DBL_MAX, +inf) stays DBL_MAX.  This clamps the order-preserving accumulator `raw` of a MIN
+ * (identity I64_MAX) or MAX (identity I64_MIN) the same way; the result is the init value exactly when the clamp bites. */
+B2Q_HD int64_t b2q_clamp_ord(int64_t raw, int64_t identity, bool as_float) {
+  const double lim = as_float ? (double)FLT_MAX : DBL_MAX;
+  int64_t b;
+  if (identity == B2Q_I64_MAX) { memcpy(&b, &lim, 8); const int64_t o = b2q_f64_to_ord(b); return raw < o ? raw : o; }
+  const double neg = -lim;
+  memcpy(&b, &neg, 8);
+  const int64_t o = b2q_f64_to_ord(b);
+  return raw > o ? raw : o;
+}
 
 B2Q_HD int64_t b2q_acc_identity(int op) {
   switch (op) {

@@ -196,7 +196,7 @@ __global__ void b2q_k_materialize(const __grid_constant__ MatArgs A) {
             const int64_t raw = A.accs[sl.acc][i];
             bool is_null = false;
             if (sl.nn >= 0) is_null = A.accs[sl.nn][i] == 0;
-            else if (sl.nn == -2) is_null = raw == sl.identity;
+            else if (sl.nn == -2) is_null = raw == sl.identity || (sl.clamp_init && b2q_clamp_ord(raw, sl.identity, sl.as_float) != raw);
             val = is_null ? sl.init_val : (sl.kind == SLOT_VALUE_ORD ? b2q_ord_to_f64(raw) : (sl.scale_day ? raw * 86400 : raw));
             if (sl.as_float && !is_null) /* agg_*_float: 32 bits written, the slot's high word still holds the init pattern's */
               val = (sl.init_val & (int64_t)0xFFFFFFFF00000000ll) | (int64_t)(uint32_t)__float_as_int((float)__longlong_as_double(val));

@@ -1612,6 +1612,7 @@ class Planner {
           sl.as_float = d.arg_type.is_float() ? 1 : 0;
           sl.acc = find_or_add_acc(q, make_acc(q, op, &d));
           sl.identity = b2q_acc_identity(op);
+          sl.clamp_init = fp && !d.skip_null ? 1 : 0; /* agg_min_double(DBL_MAX, NaN or +inf) keeps DBL_MAX; the _skip_val form assigns */
           sl.scale_day = is_days(d.arg_col) ? 1 : 0;
           /* "no value seen" <=> the accumulator still holds its identity.  Exact except for a nullable BIGINT MIN
            * whose only non-NULL values are INT64_MAX (the identity is a legal value there): that case counts. */

@@ -68,8 +68,8 @@ __device__ __forceinline__ void global_acc_raw(int op, int64_t* slot, int64_t v)
     case ACC_SUM_F64: red_add_f64(slot, __longlong_as_double(v)); break;
     case ACC_MIN_I64: red_min_s64(slot, v); break;
     case ACC_MAX_I64: red_max_s64(slot, v); break;
-    case ACC_MIN_F64: { const double d = __longlong_as_double(v); if (d == d) red_min_s64(slot, b2q_f64_to_ord(v)); break; }
-    case ACC_MAX_F64: { const double d = __longlong_as_double(v); if (d == d) red_max_s64(slot, b2q_f64_to_ord(v)); break; }
+    case ACC_MIN_F64: red_min_s64(slot, b2q_f64_min_ord(v)); break;
+    case ACC_MAX_F64: red_max_s64(slot, b2q_f64_max_ord(v)); break;
     default: break;
   }
 }
@@ -129,8 +129,8 @@ __device__ __forceinline__ void smem_acc_raw(int op, int64_t* slot, int64_t v) {
     case ACC_SUM_F64: atomicAdd(reinterpret_cast<double*>(slot), __longlong_as_double(v)); break;
     case ACC_MIN_I64: if (v < *reinterpret_cast<volatile long long*>(slot)) atomicMin(reinterpret_cast<long long*>(slot), (long long)v); break;
     case ACC_MAX_I64: if (v > *reinterpret_cast<volatile long long*>(slot)) atomicMax(reinterpret_cast<long long*>(slot), (long long)v); break;
-    case ACC_MIN_F64: { const double d = __longlong_as_double(v); if (d == d) { const long long o = b2q_f64_to_ord(v); if (o < *reinterpret_cast<volatile long long*>(slot)) atomicMin(reinterpret_cast<long long*>(slot), o); } break; }
-    case ACC_MAX_F64: { const double d = __longlong_as_double(v); if (d == d) { const long long o = b2q_f64_to_ord(v); if (o > *reinterpret_cast<volatile long long*>(slot)) atomicMax(reinterpret_cast<long long*>(slot), o); } break; }
+    case ACC_MIN_F64: { const long long o = b2q_f64_min_ord(v); if (o < *reinterpret_cast<volatile long long*>(slot)) atomicMin(reinterpret_cast<long long*>(slot), o); break; }
+    case ACC_MAX_F64: { const long long o = b2q_f64_max_ord(v); if (o > *reinterpret_cast<volatile long long*>(slot)) atomicMax(reinterpret_cast<long long*>(slot), o); break; }
     default: break;
   }
 }

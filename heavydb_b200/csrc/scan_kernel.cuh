@@ -446,8 +446,8 @@ __device__ __forceinline__ void global_update(int op, int64_t* arr, uint8_t* fla
     case ACC_SUM_F64: red_add_f64(arr + e, __longlong_as_double(v)); break;
     case ACC_MIN_I64: red_min_s64(arr + e, v); break;
     case ACC_MAX_I64: red_max_s64(arr + e, v); break;
-    case ACC_MIN_F64: { const double d = __longlong_as_double(v); if (d == d) red_min_s64(arr + e, b2q_f64_to_ord(v)); break; }
-    default: { const double d = __longlong_as_double(v); if (d == d) red_max_s64(arr + e, b2q_f64_to_ord(v)); break; }
+    case ACC_MIN_F64: red_min_s64(arr + e, b2q_f64_min_ord(v)); break;
+    default: red_max_s64(arr + e, b2q_f64_max_ord(v)); break;
   }
 }
 
@@ -480,11 +480,7 @@ __device__ __forceinline__ void smem_sum_i64(int8_t* tab, int64_t* garr, uint32_
 
 __device__ __forceinline__ void smem_minmax(int op, int8_t* tab, uint32_t e, int64_t v) {
   const bool fp = (op == ACC_MIN_F64) | (op == ACC_MAX_F64);
-  if (fp) {
-    const double d = __longlong_as_double(v);
-    if (d != d) return; /* std::min/std::max never pick up a NaN argument (RuntimeFunctions.cpp:1456-1466) */
-    v = b2q_f64_to_ord(v);
-  }
+  if (fp) v = op == ACC_MIN_F64 ? b2q_f64_min_ord(v) : b2q_f64_max_ord(v); /* a NaN loses to every number (b2q_f64_min_ord) */
   long long* p = reinterpret_cast<long long*>(tab) + e;
   const long long cur = *reinterpret_cast<volatile long long*>(p);
   if ((op == ACC_MIN_I64) | (op == ACC_MIN_F64)) { if (v < cur) atomicMin(p, (long long)v); }
@@ -1049,7 +1045,7 @@ __device__ __forceinline__ void process_chunk(const ScanArgs& A, const int8_t* c
           for (int j = 0; j < R; ++j) {
             if (!(m >> j & 1)) continue;
             int64_t x = v[j];
-            if (fp) { const double d = __longlong_as_double(x); if (d != d) continue; x = b2q_f64_to_ord(x); }
+            if (fp) x = is_min ? b2q_f64_min_ord(x) : b2q_f64_max_ord(x);
             r = is_min ? min(r, x) : max(r, x);
           }
           r = is_min ? warp_min_i64(r) : warp_max_i64(r);

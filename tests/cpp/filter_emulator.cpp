@@ -227,8 +227,8 @@ static int32_t run_program_impl(const B2QQuery* q, int32_t n_frags, const void* 
           case ACC_SUM_F64: fsum[a][e] += as_double(v); break;
           case ACC_MIN_I64: acc = v < acc ? v : acc; break;
           case ACC_MAX_I64: acc = v > acc ? v : acc; break;
-          case ACC_MIN_F64: { const int64_t o = b2q_f64_to_ord(v); acc = o < acc ? o : acc; break; }
-          case ACC_MAX_F64: { const int64_t o = b2q_f64_to_ord(v); acc = o > acc ? o : acc; break; }
+          case ACC_MIN_F64: { const int64_t o = b2q_f64_min_ord(v); acc = o < acc ? o : acc; break; }
+          case ACC_MAX_F64: { const int64_t o = b2q_f64_max_ord(v); acc = o > acc ? o : acc; break; }
           default: return -2;
         }
       }
@@ -287,7 +287,7 @@ static int32_t run_program_impl(const B2QQuery* q, int32_t n_frags, const void* 
             const int64_t raw = accs[sl.acc][i];
             bool is_null = false;
             if (sl.nn >= 0) is_null = accs[sl.nn][i] == 0;
-            else if (sl.nn == -2) is_null = raw == sl.identity;
+            else if (sl.nn == -2) is_null = raw == sl.identity || (sl.clamp_init && b2q_clamp_ord(raw, sl.identity, sl.as_float) != raw);
             val = is_null ? sl.init_val : (sl.kind == SLOT_VALUE_ORD ? b2q_ord_to_f64(raw) : (sl.scale_day ? raw * 86400 : raw));
             if (sl.as_float && !is_null) { /* as b2q_k_materialize: float image in the low word, init pattern's high word */
               const float f = static_cast<float>(as_double(val));
