@@ -444,7 +444,8 @@ struct SmemPlan {
 
 /* ---- ORDER BY / LIMIT over the materialised table (sort.cu) ------------------------------------------------ */
 #define B2Q_MAX_ORDER_ENTRIES 8
-enum { SORTKEY_I64 = 0, SORTKEY_F64 = 1, SORTKEY_AVG_I64 = 2, SORTKEY_AVG_F64 = 3 };
+/* F32 / AVG_F32: float_argument_input, the float's 4 bytes in the slot's low word */
+enum { SORTKEY_I64 = 0, SORTKEY_F64 = 1, SORTKEY_AVG_I64 = 2, SORTKEY_AVG_F64 = 3, SORTKEY_F32 = 4, SORTKEY_AVG_F32 = 5 };
 struct DevSortKey {        /* one Analyzer::OrderEntry resolved against the output layout */
   int64_t off1, off2;      /* slot offsets (row-wise: inside the row; columnar: of the column); off2 = AVG's count slot */
   int64_t null_pattern;    /* null_val_bit_pattern of the compact type (ResultSet::isNull, ResultSetIteration.cpp:2601-2618) */
@@ -452,7 +453,8 @@ struct DevSortKey {        /* one Analyzer::OrderEntry resolved against the outp
   int8_t kind;             /* SORTKEY_* */
   int8_t nullable;         /* !get_compact_type(target).get_notnull() */
   int8_t is_desc, nulls_first;
-  int8_t pad_[3];
+  int8_t scale;            /* AVG of a DECIMAL: pair_to_double divides by count x 10^scale */
+  int8_t pad_[2];
 };
 struct DevSortLayout {     /* what the kernels need to address an entry of a reference-layout buffer */
   int64_t row_size, entry_count;

@@ -909,12 +909,16 @@ static DevSortKey sort_key_of(const B2QPlan& p, const B2QOrderEntry& oe) {
   k.is_desc = oe.is_desc;
   k.nulls_first = oe.nulls_first;
   if (t.is_agg && t.agg_kind == B2Q_kAVG) {
-    k.kind = t.sql_type.type == B2Q_kDOUBLE ? SORTKEY_AVG_F64 : SORTKEY_AVG_I64;
+    k.kind = t.sql_type.type == B2Q_kDOUBLE ? SORTKEY_AVG_F64 : t.sql_type.type == B2Q_kFLOAT ? SORTKEY_AVG_F32 : SORTKEY_AVG_I64;
+    k.scale = static_cast<int8_t>(b2q_is_decimal(t.sql_type.type) ? t.sql_type.scale : 0);
     k.off2 = p.slot_offset[s + 1];
   } else if (compact.type == B2Q_kDOUBLE) {
     k.kind = SORTKEY_F64;
     const double nd = DBL_MIN;
     memcpy(&k.null_pattern, &nd, 8);
+  } else if (compact.type == B2Q_kFLOAT) {
+    k.kind = SORTKEY_F32;
+    k.null_pattern = b2q_null_bits(B2Q_kFLOAT);
   } else {
     k.kind = SORTKEY_I64;
     k.null_pattern = b2q_int_null(compact.type);
@@ -1936,8 +1940,14 @@ int32_t b2q_rs_sort(B2QResultSet* rs, const B2QOrderEntry* order_entries, int32_
   if (!rs || (n_entries && !order_entries)) return set_err(B2Q_ERR_INVALID_ARGUMENT, "null argument");
   if (n_entries < 0 || n_entries > B2Q_MAX_ORDER_ENTRIES) return set_err(B2Q_ERR_UNSUPPORTED, "more ORDER BY entries than the path carries");
   const B2QPlan& plan = rs->q.plan;
-  for (int i = 0; i < n_entries; ++i)
+  for (int i = 0; i < n_entries; ++i) {
     if (order_entries[i].tle_no < 1 || order_entries[i].tle_no > plan.num_targets) return set_err(B2Q_ERR_INVALID_ARGUMENT, "order entry refers to a target that does not exist");
+    /* ResultSet::sort orders dictionary strings through the dictionary (ResultSet.cpp:1424-1436), which this path does not hold */
+    const B2QTargetInfo& t = plan.targets[order_entries[i].tle_no - 1];
+    const bool minmax = t.is_agg && t.agg_arg_type.type != 0 && (t.agg_kind == B2Q_kMIN || t.agg_kind == B2Q_kMAX);
+    if (b2q_is_dict_string(minmax ? t.agg_arg_type.type : t.sql_type.type))
+      return set_err(B2Q_ERR_UNSUPPORTED, "ORDER BY a dictionary-encoded string needs the dictionary");
+  }
   if (!have_device()) return set_err(B2Q_ERR_NO_DEVICE, "no CUDA device visible; this path has no CPU fallback");
   rs->perm.clear();
   rs->cursor = 0; rs->fetched = 0;

@@ -943,7 +943,8 @@ class Planner {
       bool null_check = false;
       if (nullable) {
         if (negate) null_check = true;                      /* v != k must still fail for NULL */
-        else if (lo <= hi && lo <= nullv && nullv <= hi) lo = nullv + 1; /* NULL is the type's minimum: cut it off the range */
+        /* cut NULL off the range at the end where it lies: the signed minimum, or the unsigned maximum of a DICT(8|16) id */
+        else if (lo <= hi && lo <= nullv && nullv <= hi) { if (phys_unsigned(l.col_id)) hi = nullv - 1; else lo = nullv + 1; }
       }
       if (lo > hi) { /* never in range: encode as "always in range" with the negation flipped */
         t.lo = 0;

@@ -125,8 +125,10 @@ __global__ void b2q_k_sort_compact(const DevSortLayout L, const int8_t* __restri
 
 /* ---- 2. sort keys ------------------------------------------------------------------------------------------- */
 __device__ __forceinline__ double avg_of(const DevSortKey& K, int64_t sum, int64_t cnt) { /* pair_to_double, ResultSetBufferAccessors.h:197-227 */
-  const double dividend = K.kind == SORTKEY_AVG_F64 ? __longlong_as_double(sum) : (double)sum;
-  return dividend / (double)cnt;
+  const double dividend = K.kind == SORTKEY_AVG_F64   ? __longlong_as_double(sum)
+                          : K.kind == SORTKEY_AVG_F32 ? (double)__int_as_float((int32_t)sum)
+                                                      : (double)sum;
+  return K.scale ? dividend / ((double)cnt * b2q_exp_to_scale(K.scale)) : dividend / (double)cnt;
 }
 __device__ __forceinline__ uint64_t f64_key(double d) {
   if (d == 0.0) d = 0.0; /* -0.0 and +0.0 compare equal in the reference's `<` */
@@ -143,13 +145,17 @@ __global__ void b2q_k_sort_make_keys(const DevSortLayout L, const DevSortKey K, 
     const int64_t v = read_slot(L, buf, e, K.off1, K.w1);
     bool is_null = false;
     uint64_t key;
-    if (K.kind == SORTKEY_AVG_I64 || K.kind == SORTKEY_AVG_F64) {
+    if (K.kind == SORTKEY_AVG_I64 || K.kind == SORTKEY_AVG_F64 || K.kind == SORTKEY_AVG_F32) {
       const int64_t cnt = read_slot(L, buf, e, K.off2, 8);
       is_null = K.nullable && cnt == 0; /* ResultSet::isNull for a pair: !val.i2 */
       key = f64_key(cnt == 0 ? 2.2250738585072014e-308 /* NULL_DOUBLE */ : avg_of(K, v, cnt));
     } else if (K.kind == SORTKEY_F64) {
       is_null = K.nullable && v == K.null_pattern;
       key = f64_key(__longlong_as_double(v));
+    } else if (K.kind == SORTKEY_F32) { /* the slot's high word is not part of the value */
+      const int32_t b = (int32_t)v;
+      is_null = K.nullable && b == (int32_t)K.null_pattern;
+      key = f64_key((double)__int_as_float(b)); /* widened exactly: the order of the floats */
     } else {
       is_null = K.nullable && v == K.null_pattern;
       key = (uint64_t)v ^ 0x8000000000000000ull;

@@ -506,7 +506,9 @@ const B2QPlan* b2q_rs_query_mem_desc(const B2QResultSet* rs); /* getQueryMemDesc
 double b2q_rs_kernel_ms(const B2QResultSet* rs);
 /* ResultSet::sort(order_entries, top_n) (ResultSet.h:279, ResultSet.cpp:781-849) followed by iteration in sorted
  * order; top_n == 0 sorts everything.  dropFirstN / keepFirstN are SQL OFFSET / LIMIT (ResultSet.cpp:58-66).
- * The sort runs on the device (sort.cu); ties keep ascending entry order. */
+ * The sort runs on the device (sort.cu); ties keep ascending entry order.  FLOAT targets order by the float's value,
+ * AVG as pair_to_double (DECIMAL scale included); a dictionary-encoded string target is refused with B2Q_ERR_UNSUPPORTED
+ * (the reference orders it by string, through the dictionary). */
 /* ResultSet::getNDVEstimator (CardinalityEstimator.cpp:33-52) of an estimator query: -total_bits * ln(unset/total),
  * 1 for an empty bitmap, 0 when every bit is set; b2q_rs_estimator_buffer = getHostEstimatorBuffer(). */
 size_t b2q_rs_get_ndv_estimator(const B2QResultSet* rs);
