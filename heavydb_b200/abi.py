@@ -43,7 +43,7 @@ ERR_CUDA = 1004
 ERR_KEY_OUT_OF_RANGE = 1005
 
 COMM_ID_BYTES = 128
-ABI_VERSION = 7   # B2Q_ABI_VERSION of include/b2q.h this mirror was written against
+ABI_VERSION = 8   # B2Q_ABI_VERSION of include/b2q.h this mirror was written against
 EXPR_COLUMN_VAR, EXPR_CONSTANT, EXPR_BIN_OPER, EXPR_AGG, EXPR_UOPER = 1, 2, 3, 4, 5
 CPU_LEVEL, GPU_LEVEL = 1, 2
 DEVICE_CPU, DEVICE_GPU = 0, 1
@@ -52,7 +52,10 @@ DT_INT64, DT_FLOAT64, DT_UINT8 = 0, 1, 2
 RED_SUM, RED_MIN, RED_MAX, RED_BOR = 0, 1, 2, 3
 # b2q_rs_stat
 (STAT_FRAGMENTS_SCANNED, STAT_FRAGMENTS_SKIPPED, STAT_KERNEL_LAUNCHES, STAT_H2D_BYTES, STAT_SORT_US, STAT_HOST_SETUP_US,
- STAT_HOST_STREAM_US, STAT_HOST_TEARDOWN_US, STAT_RESULT_D2H_BYTES, STAT_ROWS_SCANNED) = range(10)
+ STAT_HOST_STREAM_US, STAT_HOST_TEARDOWN_US, STAT_RESULT_D2H_BYTES, STAT_ROWS_SCANNED, STAT_JOIN_TABLE) = range(11)
+# values of STAT_JOIN_TABLE: the join table the scan probed (b2q.h B2Q_JOIN_TABLE_*)
+(JOIN_TABLE_NONE, JOIN_TABLE_CALLER, JOIN_TABLE_INT32_HBM, JOIN_TABLE_INT2_HBM, JOIN_TABLE_INT32_SMEM, JOIN_TABLE_INT2_SMEM,
+ JOIN_TABLE_UINT16_SMEM) = range(7)
 
 MAX_SLOTS = 16
 MAX_TARGETS = 16

@@ -266,6 +266,7 @@ struct B2QResultSet {
   double host_setup_us = 0, host_stream_us = 0, host_teardown_us = 0;
   int64_t launches = 0, frags_scanned = 0, frags_skipped = 0;
   int64_t rows_scanned = 0; /* B2Q_STAT_ROWS_SCANNED */
+  int32_t join_table = B2Q_JOIN_TABLE_NONE; /* B2Q_STAT_JOIN_TABLE */
   bool heap_buf = false; /* b2q_rs_create_from_storage: a plain heap copy of the caller's buffer (no device involved) */
   ~B2QResultSet() {
     if (heap_buf) free(buf); else pinned_cache().put(buf, buf_cap);
@@ -706,6 +707,15 @@ static bool skip_fragment(const B2QExecUnit& u, const B2QTableInfo& tbl, const B
   return false;
 }
 
+/* B2Q_STAT_JOIN_TABLE of a query as prepared for its scan (prepare_join / choose_kernel) */
+static int32_t join_table_kind(const B2QQuery& q) {
+  if (q.prog.join.fk_col < 0) return B2Q_JOIN_TABLE_NONE;
+  const bool packed = q.prog.join.packed_col >= 0;
+  if (q.smem.join_off < 0) return packed ? B2Q_JOIN_TABLE_INT2_HBM : B2Q_JOIN_TABLE_INT32_HBM;
+  return q.prog.join.slot16 ? B2Q_JOIN_TABLE_UINT16_SMEM : packed ? B2Q_JOIN_TABLE_INT2_SMEM : B2Q_JOIN_TABLE_INT32_SMEM;
+}
+static thread_local int32_t g_launch_join_table = B2Q_JOIN_TABLE_NONE; /* b2q_last_launch_stat */
+
 /* The join level: inner-table columns to the device (they are small: dimension tables) and the one-to-one table
  * built there (PerfectJoinHashTable::reify -> initHashTableOnGpu / fill_hash_join_buff on the device). */
 static int32_t prepare_join(B2QPartial& p, const B2QExecUnit& u, cudaStream_t st) {
@@ -1063,6 +1073,7 @@ static int32_t finalize_core(B2QPartial* p, cudaStream_t st, B2QResultSet** out)
   rs->launches = p->launches + 2; /* + b2q_k_init + b2q_k_materialize */
   rs->frags_scanned = p->frags_scanned;
   rs->frags_skipped = p->frags_skipped;
+  rs->join_table = join_table_kind(p->q);
   const size_t nbytes = static_cast<size_t>(p->q.plan.buffer_size);
   if (p->q.plan.query_desc_type == B2Q_Estimator) { /* the result is the bitmap itself (ResultSet::getHostEstimatorBuffer) */
     rs->launches = p->launches + 1; /* + b2q_k_init */
@@ -1731,6 +1742,7 @@ int32_t b2q_launch(const B2QQuery* query, const B2QParams* prm, void* stream) {
     if (prm->total_matched) CU(cudaMemcpy(prm->total_matched, &matched, sizeof(int32_t), cudaMemcpyDefault));
     const int32_t ok = 0;
     if (prm->error_codes) CU(cudaMemcpy(prm->error_codes, &ok, sizeof(int32_t), cudaMemcpyDefault));
+    g_launch_join_table = B2Q_JOIN_TABLE_NONE; /* projections have no join level */
     return B2Q_OK;
   }
   B2QPartial p;
@@ -1771,6 +1783,7 @@ int32_t b2q_launch(const B2QQuery* query, const B2QParams* prm, void* stream) {
   CU(cudaMemcpyAsync(&dev_err, p.d_error, sizeof(int32_t), cudaMemcpyDeviceToHost, st));
   CU(cudaStreamSynchronize(st));
   if (prm->error_codes) cudaMemcpy(prm->error_codes, &dev_err, sizeof(int32_t), cudaMemcpyDefault);
+  if (!dev_err) g_launch_join_table = has_join ? B2Q_JOIN_TABLE_CALLER : B2Q_JOIN_TABLE_NONE;
   return dev_err;
 }
 
@@ -1998,9 +2011,11 @@ int64_t b2q_rs_stat(const B2QResultSet* rs, int32_t which) {
     case B2Q_STAT_HOST_TEARDOWN_US: return static_cast<int64_t>(rs->host_teardown_us);
     case B2Q_STAT_RESULT_D2H_BYTES: return rs->d2h_bytes;
     case B2Q_STAT_ROWS_SCANNED: return rs->rows_scanned;
+    case B2Q_STAT_JOIN_TABLE: return rs->join_table;
     default: return -1;
   }
 }
+int64_t b2q_last_launch_stat(int32_t which) { return which == B2Q_STAT_JOIN_TABLE ? g_launch_join_table : -1; }
 void b2q_rs_free(B2QResultSet* rs) { delete rs; }
 
 /* A ResultSet over storage the caller already holds: ResultSet(targets, device_type, query_mem_desc, row_set_mem_owner, ...)

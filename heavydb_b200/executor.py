@@ -111,6 +111,8 @@ def lib():
         L.b2q_rs_free.argtypes = [C.c_void_p]
         L.b2q_rs_stat.restype = C.c_int64
         L.b2q_rs_stat.argtypes = [C.c_void_p, C.c_int32]
+        L.b2q_last_launch_stat.restype = C.c_int64
+        L.b2q_last_launch_stat.argtypes = [C.c_int32]
         L.b2q_rs_get_ndv_estimator.restype = C.c_size_t
         L.b2q_rs_get_ndv_estimator.argtypes = [C.c_void_p]
         L.b2q_rs_estimator_buffer.restype = C.c_void_p
@@ -284,7 +286,8 @@ class ResultSet:
                 "sort_us": L.b2q_rs_stat(self._h, 4), "host_setup_us": L.b2q_rs_stat(self._h, 5),
                 "host_stream_us": L.b2q_rs_stat(self._h, 6), "host_teardown_us": L.b2q_rs_stat(self._h, 7),
                 "result_d2h_bytes": L.b2q_rs_stat(self._h, abi.STAT_RESULT_D2H_BYTES),
-                "rows_scanned": L.b2q_rs_stat(self._h, abi.STAT_ROWS_SCANNED)}
+                "rows_scanned": L.b2q_rs_stat(self._h, abi.STAT_ROWS_SCANNED),
+                "join_table": L.b2q_rs_stat(self._h, abi.STAT_JOIN_TABLE)}
 
     def columnarResults(self, num_threads: int = 8, with_scale: bool = False):
         """ColumnarResults(rows, num_columns, target_types) (QueryEngine/ColumnarResults.cpp:256-392): one numpy array per

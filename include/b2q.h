@@ -37,7 +37,7 @@
 extern "C" {
 #endif
 
-#define B2Q_ABI_VERSION 7 /* 2: sort_info, join level, rte_idx, columnar, dictionary / time types, B2QPlan join fields;
+#define B2Q_ABI_VERSION 8 /* 2: sort_info, join level, rte_idx, columnar, dictionary / time types, B2QPlan join fields;
                             3: DATE_IN_DAYS chunks (negative col_encoded_sizes), column-vs-column quals, 16 filter leaves,
                                operands-before-node rule, b2q_columnar_results_*, host-phase stats;
                             4: DECIMAL / NUMERIC columns (B2QTypeInfo.scale), decimal_to_double of b2q_rs_get_next_row;
@@ -48,7 +48,8 @@ extern "C" {
                                b2q_device_columns_* (ColumnarResults in device memory, Arrow C Device export, b2q_arrow.h),
                                B2Q_STAT_RESULT_D2H_BYTES;
                             7: projection units (B2Q_Projection: column targets, no GROUP BY, B2QExecUnit.scan_limit),
-                               B2Q_STAT_ROWS_SCANNED, TOTAL_MATCHED / MAX_MATCHED of b2q_launch */
+                               B2Q_STAT_ROWS_SCANNED, TOTAL_MATCHED / MAX_MATCHED of b2q_launch;
+                            8: B2Q_STAT_JOIN_TABLE (B2Q_JOIN_TABLE_*), b2q_last_launch_stat */
 
 /* ---- SQLTypes subset (Shared/sqltypes.h:65-99) -------------------------------------------------------- */
 enum {
@@ -524,8 +525,22 @@ enum { B2Q_STAT_FRAGMENTS_SCANNED = 0, B2Q_STAT_FRAGMENTS_SKIPPED = 1 /* Executo
        B2Q_STAT_RESULT_D2H_BYTES = 8 /* result-storage bytes copied device -> host so far (0 for a result_on_device set no host
                                         accessor has read yet) */,
        B2Q_STAT_ROWS_SCANNED = 9 /* projection: rows of the chunks the projection kernel loaded (a scan limit stops it early);
-                                    0 for every other query */ };
+                                    0 for every other query */,
+       B2Q_STAT_JOIN_TABLE = 10 /* the one-to-one join table the scan probed: a B2Q_JOIN_TABLE_* value */ };
+/* Layouts of the join table.  The planner picks one from the inner key's range E = join_entry_count and the inner columns
+ * the query reads: staged into shared memory when it fits beside the group table (the group table's replicas give way
+ * first), else probed in HBM / L2.  {row, value} slots carry the first 1/2/4-byte integer inner column the query reads;
+ * uint16 slots hold only that column's value - its chunk-stats minimum (0xFFFE = NULL, 0xFFFF = no row) and are chosen
+ * when it is the only inner column read, its chunk-stats span is below 65534 and the {row, value} table does not fit.
+ * The uint16 layout trusts the inner column's chunk stats: a value outside them fails the query with
+ * B2Q_ERR_KEY_OUT_OF_RANGE, where the other layouts would have read it. */
+enum { B2Q_JOIN_TABLE_NONE = 0, B2Q_JOIN_TABLE_CALLER = 1 /* b2q_launch: the caller's int32 table, read in place */,
+       B2Q_JOIN_TABLE_INT32_HBM = 2, B2Q_JOIN_TABLE_INT2_HBM = 3, B2Q_JOIN_TABLE_INT32_SMEM = 4, B2Q_JOIN_TABLE_INT2_SMEM = 5,
+       B2Q_JOIN_TABLE_UINT16_SMEM = 6 };
 int64_t b2q_rs_stat(const B2QResultSet* rs, int32_t which);
+/* statistics of the calling thread's last successful b2q_launch (it returns no result set): B2Q_STAT_JOIN_TABLE; -1 for
+ * every other statistic */
+int64_t b2q_last_launch_stat(int32_t which);
 void b2q_rs_free(B2QResultSet* rs);
 /* ResultSet(targets, device_type, query_mem_desc, ...) + allocateStorage(buffer) (ResultSet.h:183-217): a result set over a
  * group-by buffer the caller already holds, laid out as the planned query's descriptor says (b2q_plan); the bytes are

@@ -320,3 +320,22 @@ static int32_t run_program_impl(const B2QQuery* q, int32_t n_frags, const void* 
   }
   return 0;
 }
+
+/* The join table layout the planner chose for a query, with the shared-memory sizes its choice rests on:
+ * out = {B2Q_JOIN_TABLE_* value, smem.use_smem, smem.replica_bytes, smem.replicas, smem.join_bytes}.  The value is derived
+ * from the program and the shared-memory plan the way executor.cpp's join_table_kind does. */
+extern "C" int32_t b2q_test_join_layout(const B2QQuery* q, int64_t* out) {
+  if (!q || !out) return -1;
+  const DevJoin& j = q->prog.join;
+  int64_t kind = B2Q_JOIN_TABLE_NONE;
+  if (j.fk_col >= 0) {
+    if (q->smem.join_off < 0) kind = j.packed_col >= 0 ? B2Q_JOIN_TABLE_INT2_HBM : B2Q_JOIN_TABLE_INT32_HBM;
+    else kind = j.slot16 ? B2Q_JOIN_TABLE_UINT16_SMEM : j.packed_col >= 0 ? B2Q_JOIN_TABLE_INT2_SMEM : B2Q_JOIN_TABLE_INT32_SMEM;
+  }
+  out[0] = kind;
+  out[1] = q->smem.use_smem;
+  out[2] = q->smem.replica_bytes;
+  out[3] = q->smem.replicas;
+  out[4] = q->smem.join_bytes;
+  return 0;
+}
