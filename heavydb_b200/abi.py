@@ -35,6 +35,8 @@ GroupByPerfectHash, GroupByBaselineHash, Projection, TableFunction, NonGroupedAg
 # ---- error codes -----------------------------------------------------------------------------------------
 OK = 0
 ERR_OUT_OF_SLOTS = 3
+ERR_OUT_OF_TIME = 8      # dynamic watchdog: the call's device work exceeded dynamic_watchdog_time_limit
+ERR_INTERRUPTED = 9      # runtime interrupt: b2q_interrupt on the call's token
 ERR_UNSUPPORTED = 1000
 ERR_CARDINALITY_ESTIMATION_REQUIRED = 1001
 ERR_INVALID_ARGUMENT = 1002
@@ -43,7 +45,7 @@ ERR_CUDA = 1004
 ERR_KEY_OUT_OF_RANGE = 1005
 
 COMM_ID_BYTES = 128
-ABI_VERSION = 8   # B2Q_ABI_VERSION of include/b2q.h this mirror was written against
+ABI_VERSION = 9   # B2Q_ABI_VERSION of include/b2q.h this mirror was written against
 EXPR_COLUMN_VAR, EXPR_CONSTANT, EXPR_BIN_OPER, EXPR_AGG, EXPR_UOPER = 1, 2, 3, 4, 5
 CPU_LEVEL, GPU_LEVEL = 1, 2
 DEVICE_CPU, DEVICE_GPU = 0, 1
@@ -182,6 +184,11 @@ class ExecutionOptions(C.Structure):
         ("force_kernel", C.c_int32),
         ("device_ordinal", C.c_int32),
         ("result_on_device", C.c_int32),   # 1: the result stays in device memory until a host accessor needs it
+        ("with_dynamic_watchdog", C.c_int32),
+        ("dynamic_watchdog_time_limit", C.c_uint32),   # ms
+        ("allow_runtime_query_interrupt", C.c_int32),
+        ("pad_", C.c_int32),
+        ("interrupt_token", C.c_void_p),   # const B2QInterruptToken*
     ]
 
 

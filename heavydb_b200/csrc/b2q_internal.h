@@ -415,6 +415,15 @@ B2Q_HD int64_t b2q_null_bits(int type) {
   return b2q_int_null(type);
 }
 
+/* ---- stopping a running call (B2QExecutionOptions: runtime interrupt, dynamic watchdog) --------------------------------
+ * Both pointers NULL = nothing is checked (the kernels test that once, warp-uniformly, per chunk). */
+struct DevInterrupt {
+  const volatile uint32_t* flag; /* device view of the interrupt token's flag (mapped host memory), or NULL */
+  const uint64_t* t0;            /* watchdog: %globaltimer when the call's first kernel ran (device memory), or NULL */
+  uint64_t budget_ns;            /* watchdog budget */
+};
+#define B2Q_INTERRUPT_POLL_NS 100000ull /* a CTA reads the mapped flag at most once per 100 us */
+
 /* ---- launch description handed to the kernels ----------------------------------------------------------- */
 struct DevLaunch {
   /* column table: col_ptrs[frag * n_cols + c] — device pointers (device array) */
@@ -428,6 +437,7 @@ struct DevLaunch {
   int64_t* keys;                   /* baseline: open-addressing key array (EMPTY_KEY_64 initialised) */
   int32_t* error;                  /* device int: first error code */
   const int32_t* join_buff;        /* one-to-one join table (HashJoin::getJoinHashBuffer), or nullptr */
+  DevInterrupt intr;               /* what stops the launch early (error word <- B2Q_ERR_INTERRUPTED / OUT_OF_TIME) */
 };
 
 /* chosen at plan time, needed at launch */

@@ -52,14 +52,17 @@ cudaError_t launch_join_slot16(const int32_t* rows, int64_t entry_count, const i
 cudaError_t launch_bitmap_or(uint64_t* dst, const uint64_t* gathered, int64_t words, int copies, cudaStream_t st);
 size_t sort_scratch_bytes(int64_t entries);
 cudaError_t sort_device(const DevSortLayout& L, const DevSortKey* keys, int n_keys, const int8_t* buf, int8_t* scratch,
-                        cudaStream_t st, const uint32_t** perm_out, int64_t* n_out, int* launches, int64_t top_n);
+                        cudaStream_t st, const uint32_t** perm_out, int64_t* n_out, int* launches, int64_t top_n,
+                        const volatile uint32_t* stop, bool* stopped);
 cudaError_t sort_gather(const DevSortLayout& Lin, const DevGatherCols& G, const int8_t* in, int8_t* out, const uint32_t* perm,
                         int64_t first, int64_t n_out, cudaStream_t st);
 int project_rows_per_chunk();
 cudaError_t launch_project(const B2QQuery& q, const int8_t* const* col_ptrs, const int64_t* frag_rows, const int64_t* frag_chunk_start,
                            const int64_t* frag_row_base, int n_frags, int64_t total_chunks, int64_t chunk_base, int8_t* out,
                            int64_t row_size, int64_t cap, unsigned long long* status, unsigned long long* ticket,
-                           unsigned long long* counters, cudaStream_t st);
+                           unsigned long long* counters, int32_t* error, const DevInterrupt& intr, cudaStream_t st);
+cudaError_t launch_watchdog_start(uint64_t* t0, cudaStream_t st);
+cudaError_t launch_set_error(int32_t* error, int32_t code, cudaStream_t st);
 }  // namespace b2q
 
 using namespace b2q;
@@ -148,9 +151,69 @@ struct DeviceBlock {
   }
 };
 
+/* ---- stopping a running call: interrupt token and dynamic watchdog (B2QExecutionOptions) ------------------------------
+ * The token's flag is pinned host memory, mapped into every device's address space (portable): the host stores into it, the
+ * kernels read it with a relaxed system-scope load (interrupt_poll, scan_kernel.cuh). */
+struct B2QInterruptToken {
+  uint32_t* flag = nullptr;        /* host pointer == device pointer (unified addressing) */
+};
+
+/* What one call checks, made from its B2QExecutionOptions once the call's device and stream are known.  The watchdog's start
+ * time lives in one device word written by the call's first kernel (b2q_k_watchdog_start); every checking kernel of the call
+ * compares %globaltimer with it, so the budget covers the call's device work as a whole.  Shared by the partial(s) of the call
+ * (a radix retry, a projection's pre-flight count) so that the budget does not restart. */
+struct CallInterrupt {
+  DevInterrupt dev = {};                        /* what the kernels check */
+  const volatile uint32_t* host_flag = nullptr; /* the token as the host reads it between steps */
+  bool watchdog = false;
+  uint64_t* d_t0 = nullptr;
+  int device = -1;
+  cudaStream_t stream = nullptr;
+  bool enabled() const { return dev.flag != nullptr || watchdog; }
+  bool interrupted() const { return host_flag && *host_flag; }
+  static std::shared_ptr<CallInterrupt> from(const B2QExecutionOptions* eo) {
+    auto c = std::make_shared<CallInterrupt>();
+    if (eo && eo->allow_runtime_query_interrupt && eo->interrupt_token && eo->interrupt_token->flag) {
+      c->host_flag = eo->interrupt_token->flag;
+      c->dev.flag = eo->interrupt_token->flag;
+    }
+    if (eo && eo->with_dynamic_watchdog) {
+      c->watchdog = true;
+      c->dev.budget_ns = static_cast<uint64_t>(eo->dynamic_watchdog_time_limit) * 1000000ull;
+    }
+    return c;
+  }
+  /* on the call's device, before its first kernel: the watchdog's start word (once per call) */
+  cudaError_t start(int dev_id, cudaStream_t st) {
+    if (!watchdog || d_t0) return cudaSuccess;
+    device = dev_id;
+    stream = st;
+    cudaError_t e = cudaMallocAsync(reinterpret_cast<void**>(&d_t0), sizeof(uint64_t), st);
+    if (e != cudaSuccess) { d_t0 = nullptr; return e; }
+    dev.t0 = d_t0;
+    return launch_watchdog_start(d_t0, st);
+  }
+  /* Execute.cpp:2319-2324: a query that was interrupted and also ran out of time reports INTERRUPTED */
+  int32_t resolve(int32_t rc) const {
+    if (rc == B2Q_ERR_OUT_OF_TIME && watchdog && interrupted()) return B2Q_ERR_INTERRUPTED;
+    return rc;
+  }
+  ~CallInterrupt() {
+    if (!d_t0) return;
+    int cur = -1;
+    cudaGetDevice(&cur);
+    if (cur != device) cudaSetDevice(device);
+    cudaFreeAsync(d_t0, stream);
+    if (cur >= 0 && cur != device) cudaSetDevice(cur);
+    cudaGetLastError();
+  }
+};
+static const DevInterrupt kNoInterrupt = {nullptr, nullptr, 0};
+
 struct B2QPartial {
   B2QQuery q;
   int device = 0;
+  std::shared_ptr<CallInterrupt> intr; /* never null for a partial of b2q_execute_*; null for b2q_launch */
   DeviceBlock blk;
   int64_t* accs[B2Q_MAX_ACCS] = {};
   int64_t* keys = nullptr;
@@ -462,6 +525,7 @@ static int32_t scan_device_fragments(B2QPartial& p, int nf, const std::vector<co
   L.error = p.d_error;
   L.join_buff = p.join_buff;
   L.split = p.split ? 1 : 0;
+  L.intr = p.intr ? p.intr->dev : kNoInterrupt;
   if (p.radix) {
     const int32_t rc = radix_prepare(p, L.total_chunks, st);
     if (rc != B2Q_OK) return rc;
@@ -521,7 +585,11 @@ static void collect_timings(B2QPartial& p) {
 static bool skip_fragment(const B2QExecUnit& u, const B2QTableInfo& tbl, const B2QFragmentInfo& fr, bool filter_deleted);
 
 /* host-resident table: stream the referenced columns through two staging buffer sets so that the H2D copy of
- * slice k+1 overlaps the scan of slice k (the reference does the H2D in fetchChunks, unpipelined). */
+ * slice k+1 overlaps the scan of slice k (the reference does the H2D in fetchChunks, unpipelined).
+ * With an interrupt token or a watchdog, the host waits for the scan that last used a staging set before it refills it (the
+ * stream still holds the other set's copy and scan, so the pipeline keeps its depth) and then reads the token and the call's
+ * error word as of that scan: an interrupted or timed-out call stops enqueuing copies and scans.  A stop seen only on the host
+ * goes into the device error word (launch_set_error), the way every other error of the scan travels. */
 static int32_t scan_host_table(B2QPartial& p, const B2QTableInfo& tbl, const B2QExecUnit& u, bool filter_deleted, cudaStream_t st) {
   const B2QQuery& q = p.q;
   const int nc = q.prog.n_cols;
@@ -606,9 +674,20 @@ static int32_t scan_host_table(B2QPartial& p, const B2QTableInfo& tbl, const B2Q
   }
   p.host_setup_us += us_since(t_begin);
   const auto t_stream = std::chrono::steady_clock::now();
+  const bool paced = p.intr && p.intr->enabled();
+  size_t err_cap = 0;
+  int32_t* h_err_word = paced ? reinterpret_cast<int32_t*>(pinned_cache().get(64, &err_cap)) : nullptr;
+  if (h_err_word) *h_err_word = 0;
   for (size_t i = 0; i < ns && rc == B2Q_OK; ++i) {
     Stage& s = stage[i & 1];
     const Slice& sl = slices[i];
+    if (paced && s.busy) {
+      cudaEventSynchronize(s.scanned);
+      if ((h_err_word && *h_err_word) || p.intr->interrupted()) {
+        if (!(h_err_word && *h_err_word)) launch_set_error(p.d_error, B2Q_ERR_INTERRUPTED, st);
+        break;
+      }
+    }
     if (s.busy) cudaStreamWaitEvent(copy_st, s.scanned, 0); /* the scan that used this buffer set is done */
     for (int c = 0; c < nc; ++c) {
       if (q.prog.col_inner[c]) continue;
@@ -636,6 +715,7 @@ static int32_t scan_host_table(B2QPartial& p, const B2QTableInfo& tbl, const B2Q
     L.error = p.d_error;
     L.join_buff = p.join_buff;
     L.split = p.split ? 1 : 0;
+    L.intr = p.intr ? p.intr->dev : kNoInterrupt;
     if (p.radix) {
       rc = radix_launch(p, L, st);
       if (rc != B2Q_OK) break;
@@ -644,11 +724,13 @@ static int32_t scan_host_table(B2QPartial& p, const B2QTableInfo& tbl, const B2Q
       if (e != cudaSuccess) { rc = set_err(B2Q_ERR_CUDA, std::string("scan launch: ") + cudaGetErrorString(e)); break; }
       p.launches += 1;
     }
+    if (h_err_word) cudaMemcpyAsync(h_err_word, p.d_error, sizeof(int32_t), cudaMemcpyDeviceToHost, st);
     cudaEventRecord(s.scanned, st);
     s.busy = true;
   }
   cudaStreamSynchronize(copy_st);
   cudaStreamSynchronize(st);
+  if (h_err_word) pinned_cache().put(reinterpret_cast<int8_t*>(h_err_word), err_cap);
   p.host_stream_us += us_since(t_stream);
   const auto t_down = std::chrono::steady_clock::now();
   cleanup();
@@ -784,22 +866,26 @@ static int32_t prepare_join(B2QPartial& p, const B2QExecUnit& u, cudaStream_t st
 
 static int32_t execute_partial_attempt(size_t* guess, const B2QTableInfo* tbl, const B2QExecUnit* u,
                                        const B2QCompilationOptions* co, const B2QExecutionOptions* eo, int32_t has_card,
-                                       cudaStream_t st, bool allow_radix, bool defer, B2QPartial** out);
+                                       cudaStream_t st, bool allow_radix, bool defer, const std::shared_ptr<CallInterrupt>& intr,
+                                       B2QPartial** out);
 
 static int32_t execute_partial_impl(size_t* guess, const B2QTableInfo* tbl, const B2QExecUnit* u,
                                     const B2QCompilationOptions* co, const B2QExecutionOptions* eo, int32_t has_card,
                                     cudaStream_t st, B2QPartial** out) {
-  int32_t rc = execute_partial_attempt(guess, tbl, u, co, eo, has_card, st, radix_enabled(), false, out);
+  const auto intr = CallInterrupt::from(eo);
+  int32_t rc = execute_partial_attempt(guess, tbl, u, co, eo, has_card, st, radix_enabled(), false, intr, out);
   /* a structure of the radix path was too small for this input (hash clusters longer than its overflow areas): the
    * per-row probe kernel handles anything */
-  if (rc == B2Q_RADIX_RETRY) rc = execute_partial_attempt(guess, tbl, u, co, eo, has_card, st, false, false, out);
-  return rc;
+  if (rc == B2Q_RADIX_RETRY) rc = execute_partial_attempt(guess, tbl, u, co, eo, has_card, st, false, false, intr, out);
+  return intr->resolve(rc);
 }
 
 /* what a non-zero device error word means at the boundary */
 static int32_t device_error(int32_t dev_err) {
   if (dev_err == B2Q_RADIX_RETRY) return set_err(dev_err, "radix path: retry with the probe kernel");
   if (dev_err == B2Q_ERR_UNSUPPORTED) return set_err(dev_err, "join is not one-to-one (the reference rebuilds a one-to-many table): outside this path");
+  if (dev_err == B2Q_ERR_INTERRUPTED) return set_err(dev_err, "the query was interrupted (b2q_interrupt on its token)");
+  if (dev_err == B2Q_ERR_OUT_OF_TIME) return set_err(dev_err, "the query's device work exceeded dynamic_watchdog_time_limit");
   if (dev_err) return set_err(dev_err, dev_err == B2Q_ERR_OUT_OF_SLOTS ? "group-by table is full (OUT_OF_SLOTS)" : "group or join key outside the chunk-stats range");
   return B2Q_OK;
 }
@@ -809,7 +895,8 @@ static int32_t device_error(int32_t dev_err) {
  * of work with one host wait at the end. */
 static int32_t execute_partial_attempt(size_t* guess, const B2QTableInfo* tbl, const B2QExecUnit* u,
                                        const B2QCompilationOptions* co, const B2QExecutionOptions* eo, int32_t has_card,
-                                       cudaStream_t st, bool allow_radix, bool defer, B2QPartial** out) {
+                                       cudaStream_t st, bool allow_radix, bool defer, const std::shared_ptr<CallInterrupt>& intr,
+                                       B2QPartial** out) {
   if (!tbl || !u || !co || !eo || !out) return set_err(B2Q_ERR_INVALID_ARGUMENT, "null argument");
   if (co->device_type != B2Q_DEVICE_GPU) return set_err(B2Q_ERR_UNSUPPORTED, "device_type must be GPU: this path has no CPU execution");
   std::unique_ptr<B2QPartial> p(new B2QPartial());
@@ -823,6 +910,8 @@ static int32_t execute_partial_attempt(size_t* guess, const B2QTableInfo* tbl, c
   if (!have_device()) return set_err(B2Q_ERR_NO_DEVICE, "no CUDA device visible; this path has no CPU fallback");
   if (eo->device_ordinal >= 0) CU(cudaSetDevice(eo->device_ordinal));
   CU(cudaGetDevice(&p->device));
+  p->intr = intr;
+  CU(p->intr->start(p->device, st));
   p->radix = allow_radix && eo->force_kernel != B2Q_KERNEL_BASELINE_PROBE && radix_plan(p->q, &p->rp);
   p->result_on_device = eo->result_on_device != 0 && p->q.plan.query_desc_type != B2Q_Estimator; /* the bitmap is tiny and read on the host */
   const size_t extra = tbl->memory_level == B2Q_GPU_LEVEL ? launch_table_bytes(tbl->num_fragments, p->q.prog.n_cols) : 0;
@@ -860,7 +949,9 @@ static int32_t execute_partial_attempt(size_t* guess, const B2QTableInfo* tbl, c
   rc = normalize_partial(*p, st);
   if (rc != B2Q_OK) return rc;
   g_trace.mark("scan enqueued");
-  if (defer && tbl->memory_level == B2Q_GPU_LEVEL) {
+  /* with an interrupt or a watchdog a host-resident scan defers too: a stop must reach every rank of a multi-device call
+   * through the merged error word, never as an early return that leaves the peers in a collective */
+  if (defer && (tbl->memory_level == B2Q_GPU_LEVEL || p->intr->enabled())) {
     p->h_err = reinterpret_cast<int32_t*>(pinned_cache().get(64, &p->h_err_cap));
     if (!p->h_err) return set_err(B2Q_ERR_INVALID_ARGUMENT, "out of (pinned) host memory");
     *p->h_err = 0;
@@ -986,7 +1077,7 @@ static void limit_window(const B2QQuery& q, int64_t n, int64_t* first, int64_t* 
 /* ORDER BY / LIMIT / OFFSET over a materialised device buffer laid out as rs->q.plan says: compaction of the non-empty
  * entries, sort, and a gather of the kept rows into a compact buffer, which becomes the result (rs->d_buf when on_device,
  * else copied into rs->buf).  Frees d_in (stream-ordered) and returns after the stream's work is complete. */
-static int32_t sort_keep_rows(B2QResultSet* rs, int8_t* d_in, bool on_device, int device, cudaStream_t st) {
+static int32_t sort_keep_rows(B2QResultSet* rs, int8_t* d_in, bool on_device, int device, cudaStream_t st, const CallInterrupt* intr) {
   const B2QPlan plan = rs->q.plan;
   const B2QQuery& q = rs->q;
   int8_t* d_scratch = nullptr;
@@ -1000,10 +1091,11 @@ static int32_t sort_keep_rows(B2QResultSet* rs, int8_t* d_in, bool on_device, in
   const uint32_t* d_perm = nullptr;
   int64_t n = 0, first = 0, count = 0;
   int sort_launches = 0;
+  bool stopped = false;
   if (e == cudaSuccess) e = cudaEventRecord(ev0, st);
   if (e == cudaSuccess) e = sort_device(L, keys, q.n_order, d_in, d_scratch, st, &d_perm, &n, &sort_launches,
-                                        (q.has_limit ? q.limit : 0) + q.offset);
-  if (e == cudaSuccess) {
+                                        (q.has_limit ? q.limit : 0) + q.offset, intr ? intr->host_flag : nullptr, &stopped);
+  if (e == cudaSuccess && !stopped) {
     limit_window(q, n, &first, &count);
     relayout_entries(rs->q.plan, count);
     rs->buf_size = static_cast<size_t>(rs->q.plan.buffer_size);
@@ -1034,6 +1126,7 @@ static int32_t sort_keep_rows(B2QResultSet* rs, int8_t* d_in, bool on_device, in
   if (e == cudaSuccess) { float ms = 0; if (cudaEventElapsedTime(&ms, ev0, ev1) == cudaSuccess) rs->sort_ms = ms; }
   cudaEventDestroy(ev0); cudaEventDestroy(ev1);
   if (e != cudaSuccess) { cudaGetLastError(); return set_err(B2Q_ERR_CUDA, std::string("sort/materialise: ") + cudaGetErrorString(e)); }
+  if (stopped) return set_err(B2Q_ERR_INTERRUPTED, "the query was interrupted (b2q_interrupt on its token) during ORDER BY");
   rs->sorted = true;
   rs->launches += sort_launches;
   return B2Q_OK;
@@ -1046,6 +1139,16 @@ static int32_t finalize_impl(B2QPartial* p, cudaStream_t st, B2QResultSet** out)
   if (p->deferred) {
     const int32_t rc0 = partial_enqueue_error_copy(*p, st);
     if (rc0 != B2Q_OK) return rc0;
+    if (p->intr && p->intr->enabled()) {
+      /* a call that can be stopped waits for its scan here: a stopped one neither materialises nor copies back its partial table
+       * (for 1e7 groups that copy alone is several ms of the time from the interrupt to the return) */
+      if (cudaStreamSynchronize(st) != cudaSuccess) { cudaGetLastError(); return set_err(B2Q_ERR_CUDA, "stream synchronize"); }
+      if (*p->h_err) {
+        collect_timings(*p);
+        p->deferred = false;
+        return device_error(*p->h_err);
+      }
+    }
   }
   int32_t rc = finalize_core(p, st, out);
   if (!p->deferred) return rc;
@@ -1094,7 +1197,7 @@ static int32_t finalize_core(B2QPartial* p, cudaStream_t st, B2QResultSet** out)
     CU(cudaMallocAsync(reinterpret_cast<void**>(&d_out), nbytes, st));
     cudaError_t e = launch_materialize(p->q, p->accs, p->keys, d_out, st);
     if (e != cudaSuccess) { cudaFreeAsync(d_out, st); cudaGetLastError(); return set_err(B2Q_ERR_CUDA, std::string("materialise: ") + cudaGetErrorString(e)); }
-    const int32_t rc = sort_keep_rows(rs.get(), d_out, p->result_on_device, p->device, st);
+    const int32_t rc = sort_keep_rows(rs.get(), d_out, p->result_on_device, p->device, st, p->intr.get());
     if (rc != B2Q_OK) return rc;
     *out = rs.release();
     return B2Q_OK;
@@ -1245,9 +1348,11 @@ static int32_t execute_work_unit_rank(const B2QComm* comm, size_t* guess, const 
                                       cudaStream_t st, bool finalize, B2QResultSet** out, double* kernel_ms) {
   B2QExecutionOptions eo_dev = *eo;
   if (comm) eo_dev.device_ordinal = comm->device;
+  const auto intr = CallInterrupt::from(eo);
   for (int attempt = 0; attempt < 2; ++attempt) {
     B2QPartial* p = nullptr;
-    int32_t rc = execute_partial_attempt(guess, tbl, u, co, &eo_dev, has_card, st, attempt == 0 && radix_enabled(), tbl->memory_level == B2Q_GPU_LEVEL, &p);
+    int32_t rc = execute_partial_attempt(guess, tbl, u, co, &eo_dev, has_card, st, attempt == 0 && radix_enabled(),
+                                         tbl->memory_level == B2Q_GPU_LEVEL || intr->enabled(), intr, &p);
     if (rc != B2Q_OK) return rc; /* planning errors are the same on every rank: nobody reaches the collective */
     rc = merge_partial(*p, comm, st);
     if (rc == B2Q_OK && finalize) rc = finalize_impl(p, st, out);
@@ -1258,7 +1363,7 @@ static int32_t execute_work_unit_rank(const B2QComm* comm, size_t* guess, const 
     }
     if (kernel_ms) *kernel_ms = p->scan_ms;
     delete p;
-    if (rc != B2Q_RADIX_RETRY) return rc; /* the error word was MAX-merged: every rank retries together */
+    if (rc != B2Q_RADIX_RETRY) return intr->resolve(rc); /* the error word was MAX-merged: every rank retries together */
   }
   return set_err(B2Q_ERR_CUDA, "internal: radix retry did not converge");
 }
@@ -1270,9 +1375,10 @@ static int32_t execute_work_unit_rank(const B2QComm* comm, size_t* guess, const 
 struct ProjectRun {
   int64_t written = 0, scanned = 0;
   double kernel_ms = 0;
+  int32_t error = 0; /* the launch's error word: B2Q_ERR_INTERRUPTED / OUT_OF_TIME when it was stopped */
 };
 static int32_t project_scan(const B2QQuery& q, int nf, const std::vector<const int8_t*>& cols, const std::vector<int64_t>& rows,
-                            int8_t* d_out, int64_t cap, cudaStream_t st, ProjectRun* run) {
+                            int8_t* d_out, int64_t cap, cudaStream_t st, const DevInterrupt& intr, ProjectRun* run) {
   const int64_t chunk_rows = project_rows_per_chunk();
   const int nc = q.prog.n_cols;
   std::vector<int64_t> host(static_cast<size_t>(nf) * nc + nf + nf + 1);
@@ -1288,8 +1394,8 @@ static int32_t project_scan(const B2QQuery& q, int nf, const std::vector<const i
   int8_t* blk = nullptr;
   CU(cudaMallocAsync(reinterpret_cast<void**>(&blk), tab_bytes + status_bytes + 256, st));
   unsigned long long* status = reinterpret_cast<unsigned long long*>(blk + tab_bytes);
-  unsigned long long* counters = reinterpret_cast<unsigned long long*>(blk + tab_bytes + status_bytes); /* ticket, done, written, scanned */
-  unsigned long long h_counters[4] = {};
+  unsigned long long* counters = reinterpret_cast<unsigned long long*>(blk + tab_bytes + status_bytes); /* ticket, done, written, scanned, error */
+  unsigned long long h_counters[5] = {};
   cudaEvent_t ev[2] = {};
   cudaError_t e = cudaMemcpyAsync(blk, host.data(), host.size() * 8, cudaMemcpyHostToDevice, st);
   if (e == cudaSuccess) e = cudaMemsetAsync(status, 0, status_bytes + 256, st);
@@ -1300,7 +1406,8 @@ static int32_t project_scan(const B2QQuery& q, int nf, const std::vector<const i
     const int8_t* const* d_cols = reinterpret_cast<const int8_t* const*>(blk);
     const int64_t* d_rows = reinterpret_cast<const int64_t*>(blk) + static_cast<size_t>(nf) * nc;
     const int64_t row_size = q.plan.output_columnar ? 0 : q.plan.row_size;
-    e = launch_project(q, d_cols, d_rows, d_rows + nf, nullptr, nf, chunks, 0, d_out, row_size, cap, status, counters, counters + 1, st);
+    e = launch_project(q, d_cols, d_rows, d_rows + nf, nullptr, nf, chunks, 0, d_out, row_size, cap, status, counters, counters + 1,
+                       reinterpret_cast<int32_t*>(counters + 4), intr, st);
   }
   if (e == cudaSuccess) e = cudaEventRecord(ev[1], st);
   if (e == cudaSuccess) e = cudaMemcpyAsync(h_counters, counters, sizeof(h_counters), cudaMemcpyDeviceToHost, st);
@@ -1312,6 +1419,7 @@ static int32_t project_scan(const B2QQuery& q, int nf, const std::vector<const i
   if (e != cudaSuccess) { cudaGetLastError(); return set_err(e == cudaErrorMemoryAllocation ? B2Q_ERR_OUT_OF_GPU_MEM : B2Q_ERR_CUDA, std::string("projection: ") + cudaGetErrorString(e)); }
   run->written = static_cast<int64_t>(h_counters[2]);
   run->scanned = static_cast<int64_t>(h_counters[3]);
+  run->error = static_cast<int32_t>(h_counters[4]);
   return B2Q_OK;
 }
 
@@ -1321,7 +1429,7 @@ static int32_t project_scan(const B2QQuery& q, int nf, const std::vector<const i
  * and the row counters are shared, and each slice's offset words start at its first row in the fragment.  Before a staging set
  * is reused the host reads the done flag as of the scan that last used it, so a scan limit also stops the copies. */
 static int32_t project_scan_host(const B2QQuery& q, const B2QTableInfo& tbl, const std::vector<int>& frags, int8_t* d_out, int64_t cap,
-                                 cudaStream_t st, ProjectRun* run, double* h2d_bytes) {
+                                 cudaStream_t st, const CallInterrupt* intr, ProjectRun* run, double* h2d_bytes) {
   const int64_t chunk_rows = project_rows_per_chunk();
   const int64_t slice_rows = int64_t(1) << 24; /* a multiple of chunk_rows */
   const int nc = q.prog.n_cols;
@@ -1341,7 +1449,7 @@ static int32_t project_scan_host(const B2QQuery& q, const B2QTableInfo& tbl, con
   /* one device block: per-slice launch tables | status words | done, written, scanned, tickets[ns] | two staging sets */
   const size_t tab_words = ns * nc + ns + 2 * ns + ns;
   const size_t tab_bytes = DeviceBlock::pad(tab_words * 8), status_bytes = DeviceBlock::pad(static_cast<size_t>(chunks) * 8),
-               ctr_bytes = DeviceBlock::pad((3 + ns) * 8);
+               ctr_bytes = DeviceBlock::pad((4 + ns) * 8); /* done, written, scanned, tickets[ns], error word */
   size_t stage_bytes = 0;
   for (int c = 0; c < nc; ++c) stage_bytes += DeviceBlock::pad(static_cast<size_t>(max_rows) * q.prog.col_width[c] + 16);
   int8_t* blk = nullptr;
@@ -1366,9 +1474,13 @@ static int32_t project_scan_host(const B2QQuery& q, const B2QTableInfo& tbl, con
   }
   const int64_t* d_tab = reinterpret_cast<const int64_t*>(blk);
   size_t pin_cap = 0;
-  unsigned long long* h_ctr = reinterpret_cast<unsigned long long*>(pinned_cache().get(64, &pin_cap)); /* [0] done as last read, [1..3] final */
+  unsigned long long* h_ctr = reinterpret_cast<unsigned long long*>(pinned_cache().get(64, &pin_cap)); /* [0] done as last read, [1..3] final, [4] error */
   if (!h_ctr) { cudaFreeAsync(blk, st); return set_err(B2Q_ERR_INVALID_ARGUMENT, "out of (pinned) host memory"); }
   h_ctr[0] = 0;
+  h_ctr[4] = 0;
+  int32_t* d_error = reinterpret_cast<int32_t*>(counters + 3 + ns);
+  const DevInterrupt dint = intr ? intr->dev : kNoInterrupt;
+  bool host_stop = false; /* the token was seen between two slices (the kernels may not have seen it) */
   cudaStream_t copy_st = nullptr;
   cudaEvent_t ready = nullptr, ev0 = nullptr, ev1 = nullptr, copied[2] = {}, scanned[2] = {};
   bool busy[2] = {false, false};
@@ -1387,7 +1499,8 @@ static int32_t project_scan_host(const B2QQuery& q, const B2QTableInfo& tbl, con
     const int k = static_cast<int>(i & 1);
     if (busy[k]) {
       e = cudaEventSynchronize(scanned[k]); /* the scan that used this set, and the read of the done flag after it */
-      if (e != cudaSuccess || h_ctr[0]) break;
+      if (e != cudaSuccess || h_ctr[0]) break; /* the scan limit was reached, or a kernel was stopped */
+      if (intr && intr->interrupted()) { host_stop = true; break; }
       e = cudaStreamWaitEvent(copy_st, scanned[k], 0);
     }
     const Slice& x = sl[i];
@@ -1402,20 +1515,26 @@ static int32_t project_scan_host(const B2QQuery& q, const B2QTableInfo& tbl, con
     if (e == cudaSuccess)
       e = launch_project(q, reinterpret_cast<const int8_t* const*>(d_tab + i * nc), d_tab + ns * nc + i, d_tab + ns * nc + ns + 2 * i,
                          d_tab + ns * nc + 3 * ns + i, 1, h_cs[2 * i + 1], x.chunk_base, d_out, row_size, cap, status, counters + 3 + i,
-                         counters, st);
+                         counters, d_error, dint, st);
     if (e == cudaSuccess) e = cudaMemcpyAsync(h_ctr, counters, 8, cudaMemcpyDeviceToHost, st);
     if (e == cudaSuccess) e = cudaEventRecord(scanned[k], st);
     busy[k] = true;
   }
   if (e == cudaSuccess) e = cudaEventRecord(ev1, st);
   if (e == cudaSuccess) e = cudaMemcpyAsync(h_ctr + 1, counters, 3 * 8, cudaMemcpyDeviceToHost, st);
+  if (e == cudaSuccess) e = cudaMemcpyAsync(h_ctr + 4, d_error, sizeof(int32_t), cudaMemcpyDeviceToHost, st);
   cudaFreeAsync(blk, st);
   if (e == cudaSuccess) e = cudaStreamSynchronize(st);
   if (copy_st) { cudaStreamSynchronize(copy_st); cudaStreamDestroy(copy_st); }
   float ms = 0;
   if (e == cudaSuccess && cudaEventElapsedTime(&ms, ev0, ev1) == cudaSuccess) run->kernel_ms = ms;
   for (cudaEvent_t x : {ready, ev0, ev1, copied[0], copied[1], scanned[0], scanned[1]}) if (x) cudaEventDestroy(x);
-  if (e == cudaSuccess) { run->written = static_cast<int64_t>(h_ctr[2]); run->scanned = static_cast<int64_t>(h_ctr[3]); }
+  if (e == cudaSuccess) {
+    run->written = static_cast<int64_t>(h_ctr[2]);
+    run->scanned = static_cast<int64_t>(h_ctr[3]);
+    run->error = static_cast<int32_t>(h_ctr[4]);
+    if (!run->error && host_stop) run->error = B2Q_ERR_INTERRUPTED;
+  }
   pinned_cache().put(reinterpret_cast<int8_t*>(h_ctr), pin_cap);
   if (e != cudaSuccess) { cudaGetLastError(); return set_err(e == cudaErrorMemoryAllocation ? B2Q_ERR_OUT_OF_GPU_MEM : B2Q_ERR_CUDA, std::string("projection (host table): ") + cudaGetErrorString(e)); }
   return B2Q_OK;
@@ -1445,7 +1564,8 @@ static cudaError_t projection_compact(const B2QPlan& at_cap, const B2QPlan& at_n
 
 /* COUNT(*) over the quals of a projection unit: the pre-flight that sizes a projection without a scan limit */
 static int32_t projection_count(const B2QTableInfo* tbl, const B2QExecUnit* u, const B2QCompilationOptions* co,
-                                const B2QExecutionOptions* eo, cudaStream_t st, int64_t* count, double* h2d_bytes) {
+                                const B2QExecutionOptions* eo, cudaStream_t st, const std::shared_ptr<CallInterrupt>& intr,
+                                int64_t* count, double* h2d_bytes) {
   std::vector<B2QExpr> exprs(u->exprs, u->exprs + u->num_exprs);
   B2QExpr cnt;
   memset(&cnt, 0, sizeof(cnt));
@@ -1470,7 +1590,7 @@ static int32_t projection_count(const B2QTableInfo* tbl, const B2QExecUnit* u, c
   ceo.output_columnar_hint = 0;
   ceo.force_kernel = 0;
   B2QPartial* p = nullptr;
-  int32_t rc = execute_partial_attempt(nullptr, tbl, &cu, co, &ceo, 0, st, false, false, &p);
+  int32_t rc = execute_partial_attempt(nullptr, tbl, &cu, co, &ceo, 0, st, false, false, intr, &p);
   if (rc != B2Q_OK) return rc;
   std::unique_ptr<B2QPartial> own(p);
   B2QResultSet* crs = nullptr;
@@ -1485,8 +1605,15 @@ static int32_t projection_count(const B2QTableInfo* tbl, const B2QExecUnit* u, c
 }
 
 /* Executor::executeWorkUnit for a projection unit (QueryDescriptionType::Projection, is_agg = false) */
+static int32_t execute_projection_impl(const B2QTableInfo* tbl, const B2QExecUnit* u, const B2QCompilationOptions* co,
+                                       const B2QExecutionOptions* eo, const std::shared_ptr<CallInterrupt>& intr, B2QResultSet** out);
 static int32_t execute_projection(const B2QTableInfo* tbl, const B2QExecUnit* u, const B2QCompilationOptions* co,
                                   const B2QExecutionOptions* eo, B2QResultSet** out) {
+  const auto intr = CallInterrupt::from(eo);
+  return intr->resolve(execute_projection_impl(tbl, u, co, eo, intr, out));
+}
+static int32_t execute_projection_impl(const B2QTableInfo* tbl, const B2QExecUnit* u, const B2QCompilationOptions* co,
+                                       const B2QExecutionOptions* eo, const std::shared_ptr<CallInterrupt>& intr, B2QResultSet** out) {
   if (!tbl || !u || !co || !eo || !out) return set_err(B2Q_ERR_INVALID_ARGUMENT, "null argument");
   if (co->device_type != B2Q_DEVICE_GPU) return set_err(B2Q_ERR_UNSUPPORTED, "device_type must be GPU: this path has no CPU execution");
   std::unique_ptr<B2QResultSet> rs(new B2QResultSet());
@@ -1501,6 +1628,7 @@ static int32_t execute_projection(const B2QTableInfo* tbl, const B2QExecUnit* u,
   CU(cudaGetDevice(&device));
   configure_pool_once(device);
   cudaStream_t st = nullptr;
+  CU(intr->start(device, st));
   const bool filter_deleted = !co->ignore_deleted_column;
   B2QQuery& q = rs->q;
   /* fragments in fragment-id order (the order resultsUnion gives per-fragment results), skipped ones left out */
@@ -1529,17 +1657,19 @@ static int32_t execute_projection(const B2QTableInfo* tbl, const B2QExecUnit* u,
   if (q.has_limit && q.limit == 0) {
     cap = 0;
   } else if (u->scan_limit == 0) {
-    rc = projection_count(tbl, u, co, eo, st, &cap, &rs->h2d_bytes);
+    rc = projection_count(tbl, u, co, eo, st, intr, &cap, &rs->h2d_bytes);
     if (rc != B2Q_OK) return rc;
     rs->launches += 2;
+    if (intr->interrupted()) return set_err(B2Q_ERR_INTERRUPTED, "the query was interrupted (b2q_interrupt on its token) after its row count");
   }
   projection_relayout(q, cap);
   const B2QPlan at_cap = q.plan;
   int8_t* d_out = nullptr;
   CU(cudaMallocAsync(reinterpret_cast<void**>(&d_out), std::max<int64_t>(at_cap.buffer_size, 8), st));
   ProjectRun run;
-  if (tbl->memory_level == B2Q_CPU_LEVEL) rc = project_scan_host(q, *tbl, scanned_frags, d_out, cap, st, &run, &rs->h2d_bytes);
-  else rc = project_scan(q, static_cast<int>(rows.size()), cols, rows, d_out, cap, st, &run);
+  if (tbl->memory_level == B2Q_CPU_LEVEL) rc = project_scan_host(q, *tbl, scanned_frags, d_out, cap, st, intr.get(), &run, &rs->h2d_bytes);
+  else rc = project_scan(q, static_cast<int>(rows.size()), cols, rows, d_out, cap, st, intr->dev, &run);
+  if (rc == B2Q_OK && run.error) rc = device_error(run.error);
   if (rc != B2Q_OK) { cudaFreeAsync(d_out, st); return rc; }
   rs->launches += rows.empty() ? 0 : 1;
   rs->scan_ms = run.kernel_ms;
@@ -1561,7 +1691,7 @@ static int32_t execute_projection(const B2QTableInfo* tbl, const B2QExecUnit* u,
   if (e != cudaSuccess) { if (d_res) cudaFreeAsync(d_res, st); cudaGetLastError(); return set_err(B2Q_ERR_CUDA, std::string("projection compaction: ") + cudaGetErrorString(e)); }
   const bool want_sort = q.n_order > 0 || q.has_limit || q.offset > 0;
   if (q.plan.buffer_size && want_sort) {
-    rc = sort_keep_rows(rs.get(), d_res, eo->result_on_device != 0, device, st);
+    rc = sort_keep_rows(rs.get(), d_res, eo->result_on_device != 0, device, st, intr.get());
     if (rc != B2Q_OK) return rc;
     *out = rs.release();
     return B2Q_OK;
@@ -1674,16 +1804,17 @@ int32_t b2q_execute_work_unit(size_t* guess, int32_t is_agg, const B2QTableInfo*
   CallerDevice restore;
   if (is_projection_unit(u) && !u->num_join_quals) return execute_projection(tbl, u, co, eo, out);
   g_trace.begin();
+  const auto intr = CallInterrupt::from(eo);
   for (int attempt = 0; attempt < 2; ++attempt) {
     B2QPartial* p = nullptr;
-    int32_t rc = execute_partial_attempt(guess, tbl, u, co, eo, has_card, nullptr, attempt == 0 && radix_enabled(), true, &p);
+    int32_t rc = execute_partial_attempt(guess, tbl, u, co, eo, has_card, nullptr, attempt == 0 && radix_enabled(), true, intr, &p);
     if (rc == B2Q_OK) {
       rc = finalize_impl(p, nullptr, out);
       g_trace.mark("finalize");
       delete p;
       g_trace.mark("release");
     }
-    if (rc != B2Q_RADIX_RETRY) { g_trace.end(); return rc; }
+    if (rc != B2Q_RADIX_RETRY) { g_trace.end(); return intr->resolve(rc); }
   }
   return set_err(B2Q_ERR_CUDA, "internal: radix retry did not converge");
 }
@@ -1736,7 +1867,7 @@ int32_t b2q_launch(const B2QQuery* query, const B2QParams* prm, void* stream) {
     CU(cudaMemcpyAsync(&d_out, prm->group_by_buffers, sizeof(int64_t*), cudaMemcpyDefault, st));
     CU(cudaStreamSynchronize(st));
     ProjectRun run;
-    const int32_t rc = project_scan(q, nf, cols, rows, reinterpret_cast<int8_t*>(d_out), cap, st, &run);
+    const int32_t rc = project_scan(q, nf, cols, rows, reinterpret_cast<int8_t*>(d_out), cap, st, kNoInterrupt, &run);
     if (rc != B2Q_OK) return rc;
     const int32_t matched = static_cast<int32_t>(std::min<int64_t>(run.written, INT32_MAX));
     if (prm->total_matched) CU(cudaMemcpy(prm->total_matched, &matched, sizeof(int32_t), cudaMemcpyDefault));
@@ -1982,7 +2113,9 @@ int32_t b2q_rs_sort(B2QResultSet* rs, const B2QOrderEntry* order_entries, int32_
   const uint32_t* d_perm = nullptr;
   int64_t n = 0;
   int launches = 0;
-  if (e == cudaSuccess) e = sort_device(L, keys, n_entries, rs->d_buf ? rs->d_buf : d_buf, d_scratch, st, &d_perm, &n, &launches, static_cast<int64_t>(top_n));
+  bool stopped = false; /* ResultSet::sort takes no interrupt token */
+  if (e == cudaSuccess) e = sort_device(L, keys, n_entries, rs->d_buf ? rs->d_buf : d_buf, d_scratch, st, &d_perm, &n, &launches, static_cast<int64_t>(top_n),
+                                        nullptr, &stopped);
   if (e == cudaSuccess) {
     const int64_t keep = top_n && static_cast<int64_t>(top_n) < n ? static_cast<int64_t>(top_n) : n;
     rs->perm.resize(static_cast<size_t>(keep));
@@ -2141,6 +2274,31 @@ int32_t b2q_execute_work_unit_multi(B2QComm* const* comms, int32_t ndev, size_t*
     }
   return B2Q_OK;
 }
+
+/* ---- runtime query interrupt ------------------------------------------------------------------------------------------ */
+int32_t b2q_interrupt_token_create(B2QInterruptToken** out) {
+  if (!out) return set_err(B2Q_ERR_INVALID_ARGUMENT, "null argument");
+  *out = nullptr;
+  if (!have_device()) return set_err(B2Q_ERR_NO_DEVICE, "no CUDA device visible: an interrupt token is device-mapped host memory");
+  std::unique_ptr<B2QInterruptToken> t(new B2QInterruptToken());
+  void* p = nullptr;
+  /* mapped: the kernels read it where it lies; portable: every device of a multi-device call reads the same word */
+  CU(cudaHostAlloc(&p, 64, cudaHostAllocMapped | cudaHostAllocPortable));
+  t->flag = static_cast<uint32_t*>(p);
+  __atomic_store_n(t->flag, 0u, __ATOMIC_RELEASE);
+  *out = t.release();
+  return B2Q_OK;
+}
+void b2q_interrupt_token_destroy(B2QInterruptToken* t) {
+  if (!t) return;
+  if (t->flag) { cudaFreeHost(t->flag); cudaGetLastError(); }
+  delete t;
+}
+/* Executor::interrupt (GpuInterrupt.cpp:33-160) sets the flag of the running query's session; this is that store */
+void b2q_interrupt(B2QInterruptToken* t) { if (t && t->flag) __atomic_store_n(t->flag, 1u, __ATOMIC_RELEASE); }
+/* Executor::resetInterrupt (GpuInterrupt.cpp:292-300) */
+void b2q_interrupt_reset(B2QInterruptToken* t) { if (t && t->flag) __atomic_store_n(t->flag, 0u, __ATOMIC_RELEASE); }
+int32_t b2q_interrupt_is_set(const B2QInterruptToken* t) { return t && t->flag && __atomic_load_n(t->flag, __ATOMIC_ACQUIRE) ? 1 : 0; }
 
 int32_t b2q_gen_column(void* dst, int32_t sql_type, uint64_t seed, uint32_t col_tag, int64_t row0, int64_t count,
                        int64_t lo, int64_t span, void* stream) {

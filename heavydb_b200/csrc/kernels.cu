@@ -360,6 +360,26 @@ cudaError_t launch_init(const B2QQuery& q, int64_t* const* accs, int64_t* keys, 
   return cudaGetLastError();
 }
 
+/* dynamic watchdog: the call's first kernel records the start of its device work (dynamic_watchdog_init, cuda_mapd_rt.cu:140-164,
+ * here %globaltimer for the whole call instead of per-SM cycle counters per launch) */
+__global__ void b2q_k_watchdog_start(uint64_t* t0) {
+  uint64_t t;
+  asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
+  *t0 = t;
+}
+cudaError_t launch_watchdog_start(uint64_t* t0, cudaStream_t st) {
+  b2q_k_watchdog_start<<<1, 1, 0, st>>>(t0);
+  return cudaGetLastError();
+}
+
+/* the host saw the interrupt between two steps: the code goes into the call's error word like a kernel's would (first error
+ * wins), so that it travels the same way, through the cross-device MAX all-reduce included */
+__global__ void b2q_k_set_error(int32_t* error, int32_t code) { atomicCAS(error, 0, code); }
+cudaError_t launch_set_error(int32_t* error, int32_t code, cudaStream_t st) {
+  b2q_k_set_error<<<1, 1, 0, st>>>(error, code);
+  return cudaGetLastError();
+}
+
 cudaError_t launch_bitmap_or(uint64_t* dst, const uint64_t* gathered, int64_t words, int copies, cudaStream_t st) {
   if (words <= 0) return cudaSuccess;
   const int64_t cap = (int64_t)sm_count() * 8;

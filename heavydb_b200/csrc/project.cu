@@ -51,6 +51,8 @@ struct ProjArgs {
   unsigned long long* status;      /* [all chunks of all launches] zero-initialised */
   unsigned long long* ticket;      /* this launch's chunk counter, zero-initialised */
   unsigned long long* counters;    /* [0] done flag, [1] rows written, [2] rows of the chunks loaded */
+  int32_t* error;                  /* B2Q_ERR_INTERRUPTED / OUT_OF_TIME when the launch was stopped */
+  DevInterrupt intr;
 };
 
 __device__ __forceinline__ void st_release(unsigned long long* p, unsigned long long v) {
@@ -94,11 +96,23 @@ __global__ void __launch_bounds__(kProjBlock) b2q_k_project(const __grid_constan
   const int64_t limit = A.proj.scan_limit > 0 ? (A.proj.scan_limit < A.cap ? A.proj.scan_limit : A.cap) : A.cap;
   unsigned long long* done = A.counters;
 
+  /* Interrupt / watchdog: the stop takes the scan limit's path.  Thread 0 polls before it claims a chunk; a stop records its
+   * code and raises the done flag, and from then on every CTA claims nothing more.  Why no CTA can then wait forever in the
+   * look-back below: a CTA only looks back over chunks with smaller tickets, i.e. chunks some CTA has already claimed, and
+   * every claimed chunk publishes a status word with a flag its successors accept as final — a chunk claimed before the
+   * done flag is processed to the end (its own look-back only waits on earlier claims, by induction), a chunk claimed after
+   * it publishes an empty aggregate (kFlagAgg | 0) at once.  Chunks never claimed have no successor that waits on them. */
+  const bool check = interrupt_enabled(A.intr);
+  PollState poll = {0, 0};
   int frag = 0;
   int64_t frag_first = 0, next_first = __ldg(A.frag_chunk_start + 1);
   for (;;) {
     if (tid == 0) {
       unsigned long long c = ~0ull;
+      if (check) {
+        const int32_t code = interrupt_poll(A.intr, A.error, poll);
+        if (code) { atomicCAS(A.error, 0, code); st_release(done, 1ull); }
+      }
       if (!ld_acquire(done)) {
         c = atomicAdd(A.ticket, 1ull);
         if (c >= (unsigned long long)A.total_chunks) c = ~0ull;
@@ -235,9 +249,11 @@ int project_rows_per_chunk() { return static_cast<int>(kProjChunk); }
 cudaError_t launch_project(const B2QQuery& q, const int8_t* const* col_ptrs, const int64_t* frag_rows, const int64_t* frag_chunk_start,
                            const int64_t* frag_row_base, int n_frags, int64_t total_chunks, int64_t chunk_base, int8_t* out,
                            int64_t row_size, int64_t cap, unsigned long long* status, unsigned long long* ticket,
-                           unsigned long long* counters, cudaStream_t st) {
+                           unsigned long long* counters, int32_t* error, const DevInterrupt& intr, cudaStream_t st) {
   ProjArgs a;
   memset(&a, 0, sizeof(a));
+  a.error = error;
+  a.intr = intr;
   a.filter = q.prog.filter;
   a.proj = q.proj;
   a.col_ptrs = col_ptrs;

@@ -254,6 +254,12 @@ __global__ void __launch_bounds__(kRadixBlock, 1) b2q_k_radix_partition(const __
   const int tid = threadIdx.x;
   constexpr int nthr = kRadixBlock;
   const int64_t chunk_rows = (int64_t)nthr * R;
+  /* interrupt / watchdog: as in b2q_k_scan (no barrier in the loop: warp 0 polls, every warp reads s_stop per chunk) */
+  __shared__ int32_t s_stop;
+  const bool check = interrupt_enabled(Lh.intr);
+  const int lane = tid & 31, warp = tid >> 5;
+  PollState poll = {0, 0};
+  if (tid == 0) s_stop = 0;
   for (int i = tid; i < A.n_parts; i += nthr) s_cnt[i] = 0;
   __syncthreads();
   uint64_t pol;
@@ -262,6 +268,17 @@ __global__ void __launch_bounds__(kRadixBlock, 1) b2q_k_radix_partition(const __
   int64_t frag_first = 0;
   int64_t next_first = __ldg(Lh.frag_chunk_start + 1);
   for (int64_t chunk = A.chunk_begin + blockIdx.x; chunk < A.chunk_end; chunk += gridDim.x) {
+    if (check) {
+      int32_t stop = 0;
+      if (lane == 0) {
+        if (warp == 0) {
+          const int32_t code = interrupt_poll(Lh.intr, Lh.error, poll);
+          if (code) { atomicCAS(Lh.error, 0, code); *reinterpret_cast<volatile int32_t*>(&s_stop) = 1; }
+        }
+        stop = *reinterpret_cast<volatile int32_t*>(&s_stop);
+      }
+      if (__shfl_sync(0xffffffffu, stop, 0)) break;
+    }
     while (chunk >= next_first) {
       ++frag;
       frag_first = next_first;
@@ -298,7 +315,13 @@ __global__ void __launch_bounds__(kRadixBlock, 1) b2q_k_radix_partition_tile(con
   uint32_t* s_off = s_cnt + NP;                                           /* [NP + 1] exclusive scan of s_cnt */
   uint16_t* s_pid = reinterpret_cast<uint16_t*>(s_off + NP + 1);          /* [TILE] partition of a tile slot */
   __shared__ uint32_t s_warp[32];
+  /* interrupt / watchdog: thread 0 polls before a chunk's rows are counted; the loop's first barrier publishes s_stop and the
+   * whole CTA leaves the loop together right after it (every later barrier of the chunk is skipped by all threads alike) */
+  __shared__ int32_t s_stop;
+  const bool check = interrupt_enabled(Lh.intr);
+  PollState poll = {0, 0};
   const int64_t chunk_rows = (int64_t)TILE;
+  if (tid == 0) s_stop = 0;
   for (int i = tid; i < NP; i += nthr) { s_cur[i] = 0; s_cnt[i] = 0; }
   __syncthreads();
   uint64_t pol;
@@ -360,7 +383,12 @@ __global__ void __launch_bounds__(kRadixBlock, 1) b2q_k_radix_partition_tile(con
       const uint32_t part = part_of_mix(mix_key(key), (uint32_t)NP);
       pr[j] = part << 16 | atomicAdd(s_cnt + part, 1u);
     }
+    if (check && tid == 0) {
+      const int32_t code = interrupt_poll(Lh.intr, Lh.error, poll);
+      if (code) { atomicCAS(Lh.error, 0, code); s_stop = 1; }
+    }
     __syncthreads();
+    if (check && s_stop) break;
     /* ---- exclusive scan of the bucket sizes ---- */
     uint32_t loc = 0;
     for (int q = 0; q < per; ++q) { const int i = tid * per + q; if (i < NP) loc += s_cnt[i]; }
@@ -485,9 +513,20 @@ __global__ void __launch_bounds__(kRadixBlock, 1) b2q_k_radix_aggregate(const __
   const bool fused_count = fused && P.accs[0].op == ACC_COUNT;
   uint64_t pol;
   asm("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(pol));
+  /* interrupt / watchdog: thread 0 polls when it claims a partition (a stop claims none: the CTA leaves at the claim's barrier)
+   * and every 8 tuple blocks of warp 0; the other warps read s_stop per tuple block and stop streaming.  The private table
+   * of a partition in progress is still merged (its barrier and merge loop run as usual); the call fails anyway. */
+  __shared__ int32_t s_stop;
+  const bool check = interrupt_enabled(Lh.intr);
+  PollState poll = {0, 0};
+  if (tid == 0) s_stop = 0;
   for (;;) {
     __syncthreads();
-    if (tid == 0) s_part = atomicAdd(A.work_counter, 1u);
+    if (tid == 0) {
+      int32_t code = 0;
+      if (check && !s_stop && (code = interrupt_poll(Lh.intr, Lh.error, poll)) != 0) { atomicCAS(Lh.error, 0, code); s_stop = 1; }
+      s_part = (check && s_stop) ? (uint32_t)A.n_parts : atomicAdd(A.work_counter, 1u);
+    }
     __syncthreads();
     const uint32_t part = s_part;
     if (part >= (uint32_t)A.n_parts) break;
@@ -551,7 +590,19 @@ __global__ void __launch_bounds__(kRadixBlock, 1) b2q_k_radix_aggregate(const __
       }
     };
     int c = 0; /* region of block b: blocks are taken in increasing order, so the region is a moving cursor */
-    for (uint32_t b = tid >> 5; b < total_blocks; b += nthr / 32) {
+    uint32_t nblk = 0;
+    for (uint32_t b = tid >> 5; b < total_blocks; b += nthr / 32, ++nblk) {
+      if (check) {
+        int32_t stop = 0;
+        if (lane == 0) {
+          if (tid == 0 && (nblk & 7u) == 0) {
+            const int32_t code = interrupt_poll(Lh.intr, Lh.error, poll);
+            if (code) { atomicCAS(Lh.error, 0, code); *reinterpret_cast<volatile int32_t*>(&s_stop) = 1; }
+          }
+          stop = *reinterpret_cast<volatile int32_t*>(&s_stop);
+        }
+        if (__shfl_sync(0xffffffffu, stop, 0)) break;
+      }
       while (s_blk[c + 1] <= b) ++c;
       const uint32_t cnt = __ldg(A.counts + (size_t)part * n_cta1 + c);
       const uint32_t off = (b - s_blk[c]) * kTupleBlock;

@@ -538,6 +538,50 @@ __device__ __forceinline__ void tma_bulk_g2s(void* smem_dst, const void* gsrc, u
 }
 
 /* ---------------------------------------------------------------------------------------------------------
+ * runtime interrupt / dynamic watchdog (check_interrupt, dynamic_watchdog: cuda_mapd_rt.cu:98-168).  ONE lane per CTA polls:
+ * it reads %globaltimer once per chunk and acts at most every B2Q_INTERRUPT_POLL_NS.  Then it compares the time with the
+ * watchdog's start word (read once per launch) and looks for a stop:
+ *   - CTA 0 reads the token's flag in mapped host memory (a relaxed system-scope load: the host's store becomes visible without
+ *     any fence on this side) and, when it is set, writes B2Q_ERR_INTERRUPTED into the call's error word;
+ *   - every other CTA reads the call's error word in device memory.
+ * (Every CTA reading the one host word was measured first: hundreds of CTAs' PCIe reads of one address queue up and the c2 scan
+ * went from 6.8 to 255 ms.  One reader per device keeps the system-memory traffic at ~10 reads per ms.)
+ * `ps` is the polling lane's state (zero before its first poll, so a token set before the call stops the first chunk).  Returns
+ * the code to stop with, 0 to go on; the caller records it with atomicCAS(error, 0, code) and shares the decision with its CTA.
+ * ------------------------------------------------------------------------------------------------------- */
+struct PollState {
+  uint64_t last; /* %globaltimer of the previous poll */
+  uint64_t t0;   /* the watchdog's start, once read */
+};
+__device__ __forceinline__ bool interrupt_enabled(const DevInterrupt& I) { return I.flag != nullptr || I.t0 != nullptr; }
+__device__ __forceinline__ uint64_t global_timer_ns() {
+  uint64_t t;
+  asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
+  return t;
+}
+static __device__ __noinline__ int32_t interrupt_poll(const DevInterrupt& I, const int32_t* error, PollState& ps) {
+  const uint64_t now = global_timer_ns();
+  if (ps.last != 0 && now - ps.last < B2Q_INTERRUPT_POLL_NS) return 0;
+  ps.last = now;
+  if (I.t0) {
+    if (!ps.t0) ps.t0 = __ldcg(reinterpret_cast<const unsigned long long*>(I.t0));
+    if (now > ps.t0 && now - ps.t0 > I.budget_ns) return B2Q_ERR_OUT_OF_TIME;
+  }
+  if (I.flag) {
+    if (blockIdx.x == 0) {
+      uint32_t f;
+      asm volatile("ld.relaxed.sys.global.u32 %0, [%1];" : "=r"(f) : "l"(I.flag) : "memory");
+      if (f) return B2Q_ERR_INTERRUPTED;
+    } else {
+      int32_t e;
+      asm volatile("ld.relaxed.gpu.global.s32 %0, [%1];" : "=r"(e) : "l"(error) : "memory");
+      if (e == B2Q_ERR_INTERRUPTED) return B2Q_ERR_INTERRUPTED;
+    }
+  }
+  return 0;
+}
+
+/* ---------------------------------------------------------------------------------------------------------
  * the scan kernel
  * ------------------------------------------------------------------------------------------------------- */
 struct ScanArgs {
@@ -1143,11 +1187,33 @@ __global__ void __launch_bounds__(BLOCK, 1024 / BLOCK) b2q_k_scan(const __grid_c
   uint64_t pol_tab;
   asm("createpolicy.fractional.L2::evict_last.b64 %0, 1.0;" : "=l"(pol_tab));
 
+  /* interrupt / watchdog: lane 0 of warp 0 polls and raises s_stop; every warp reads s_stop (lane 0, broadcast) before each
+   * chunk and leaves the loop.  The loop has no barrier, so warps may leave it a chunk apart; the epilogue's __syncthreads
+   * is reached by all of them.  s_stop needs the barrier below only when the check is on. */
+  __shared__ int32_t s_stop;
+  const bool check = interrupt_enabled(Lh.intr);
+  PollState poll = {0, 0};
+  if (check) {
+    if (tid == 0) s_stop = 0;
+    __syncthreads();
+  }
+
   /* chunks are visited in increasing order, so the owning fragment is a moving cursor, not a search */
   int frag = 0;
   int64_t frag_first = 0;                                   /* first chunk of `frag` */
   int64_t next_first = __ldg(Lh.frag_chunk_start + 1);      /* first chunk of frag + 1 */
   for (int64_t chunk = blockIdx.x; chunk < Lh.total_chunks; chunk += gridDim.x) {
+    if (check) {
+      int32_t stop = 0;
+      if (lane == 0) {
+        if (warp == 0) {
+          const int32_t code = interrupt_poll(Lh.intr, Lh.error, poll);
+          if (code) { atomicCAS(Lh.error, 0, code); *reinterpret_cast<volatile int32_t*>(&s_stop) = 1; }
+        }
+        stop = *reinterpret_cast<volatile int32_t*>(&s_stop);
+      }
+      if (__shfl_sync(0xffffffffu, stop, 0)) break;
+    }
     while (chunk >= next_first) {
       ++frag;
       frag_first = next_first;

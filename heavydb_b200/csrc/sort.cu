@@ -435,8 +435,13 @@ size_t sort_scratch_bytes(int64_t entries) {
 /* Sorts the non-empty entries of the device buffer `buf` (layout L) by `keys` (n_keys order entries).
  * Returns in *perm_out a pointer (inside `scratch`) to the sorted entry indices and in *n_out their count.
  * One stream synchronisation (the count of non-empty entries decides every later grid). */
+/* `stop` (the call's interrupt token, or NULL) is read after each of those host waits; once it is set nothing more is enqueued
+ * and *stopped says so (the permutation is then incomplete). */
 cudaError_t sort_device(const DevSortLayout& L, const DevSortKey* keys, int n_keys, const int8_t* buf, int8_t* scratch,
-                        cudaStream_t st, const uint32_t** perm_out, int64_t* n_out, int* launches, int64_t top_n) {
+                        cudaStream_t st, const uint32_t** perm_out, int64_t* n_out, int* launches, int64_t top_n,
+                        const volatile uint32_t* stop, bool* stopped) {
+  *stopped = false;
+  auto interrupted = [&]() { if (stop && *stop) *stopped = true; return *stopped; };
   const int64_t n_entries = L.entry_count;
   const size_t nblocks_c = (size_t)((n_entries + SORT_TILE - 1) / SORT_TILE);
   auto pad = [](size_t x) { return (x + 255) & ~size_t(255); };
@@ -459,7 +464,7 @@ cudaError_t sort_device(const DevSortLayout& L, const DevSortKey* keys, int n_ke
 
   cudaError_t e = compact_entries(L, buf, block_counts, perm_a, d_total, st, n_out);
   *launches += 3;
-  if (e != cudaSuccess) return e;
+  if (e != cudaSuccess || interrupted()) return e;
   uint32_t h_total = 0;
   int64_t n = *n_out; /* the number of non-empty entries, whatever is sorted below */
   if (n <= 1 || n_keys == 0) return cudaGetLastError();
@@ -478,7 +483,7 @@ cudaError_t sort_device(const DevSortLayout& L, const DevSortKey* keys, int n_ke
     b2q_k_sort_bits<<<g0, 256, 0, st>>>(keys_a, n, d_bits);
     e = cudaMemcpyAsync(hb, d_bits, 16, cudaMemcpyDeviceToHost, st);
     if (e == cudaSuccess) e = cudaStreamSynchronize(st);
-    if (e != cudaSuccess) return e;
+    if (e != cudaSuccess || interrupted()) return e;
     const unsigned long long kdiff = hb[0] ^ hb[1];
     const int msb = kdiff ? 63 - __builtin_clzll(kdiff) : 0;
     const int shift = msb > 13 ? msb - 13 : 0;
@@ -488,7 +493,7 @@ cudaError_t sort_device(const DevSortLayout& L, const DevSortKey* keys, int n_ke
     std::vector<uint32_t> h16(65536);
     e = cudaMemcpyAsync(h16.data(), hist16, 65536 * 4, cudaMemcpyDeviceToHost, st);
     if (e == cudaSuccess) e = cudaStreamSynchronize(st);
-    if (e != cudaSuccess) return e;
+    if (e != cudaSuccess || interrupted()) return e;
     uint32_t max_bucket = 65535;
     int64_t cum = 0;
     for (uint32_t b = 0; b < 65536; ++b) { cum += h16[b]; if (cum >= top_n) { max_bucket = b; break; } }
@@ -499,7 +504,7 @@ cudaError_t sort_device(const DevSortLayout& L, const DevSortKey* keys, int n_ke
       *launches += 3;
       e = cudaMemcpyAsync(&h_total, d_total, 4, cudaMemcpyDeviceToHost, st);
       if (e == cudaSuccess) e = cudaStreamSynchronize(st);
-      if (e != cudaSuccess) return e;
+      if (e != cudaSuccess || interrupted()) return e;
       std::swap(pin, pout);
       n = h_total; /* >= top_n survivors, in ascending entry order */
     }
@@ -527,7 +532,7 @@ cudaError_t sort_device(const DevSortLayout& L, const DevSortKey* keys, int n_ke
     *launches += 1;
     e = cudaMemcpyAsync(h_bits, d_bits, 16, cudaMemcpyDeviceToHost, st);
     if (e == cudaSuccess) e = cudaStreamSynchronize(st);
-    if (e != cudaSuccess) return e;
+    if (e != cudaSuccess || interrupted()) return e;
     const unsigned long long diff = h_bits[0] ^ h_bits[1];
     for (int shift = 0; shift < 64; shift += 8) if ((diff >> shift) & 255ull) radix_pass(shift);
     if (keys[k].nullable) {

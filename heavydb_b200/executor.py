@@ -170,6 +170,13 @@ def lib():
         L.b2q_device_columns_export_arrow.argtypes = [C.c_void_p, C.POINTER(C.c_char_p), C.POINTER(abi.ArrowSchema),
                                                       C.POINTER(abi.ArrowDeviceArray)]
         L.b2q_device_columns_free.argtypes = [C.c_void_p, C.c_void_p]
+        L.b2q_interrupt_token_create.restype = C.c_int32
+        L.b2q_interrupt_token_create.argtypes = [C.POINTER(C.c_void_p)]
+        for n in ("b2q_interrupt_token_destroy", "b2q_interrupt", "b2q_interrupt_reset"):
+            getattr(L, n).restype = None
+            getattr(L, n).argtypes = [C.c_void_p]
+        L.b2q_interrupt_is_set.restype = C.c_int32
+        L.b2q_interrupt_is_set.argtypes = [C.c_void_p]
         if L.b2q_abi_version() != abi.ABI_VERSION:
             raise ImportError("libb2q.so ABI version mismatch")
         _lib = L
@@ -187,6 +194,41 @@ def _raise(code: int):
     raise QueryExecutionError(code, msg)
 
 
+def resolve_interrupt_error(code: int, with_dynamic_watchdog: bool, interrupted: bool) -> int:
+    """The error a stopped call reports (Execute.cpp:2319-2324): a query that was interrupted and also ran out of time
+    reports INTERRUPTED.  libb2q applies the same rule before it returns; this restates it for callers that combine
+    codes themselves (e.g. the ranks of a multi-process query)."""
+    if code == abi.ERR_OUT_OF_TIME and with_dynamic_watchdog and interrupted:
+        return abi.ERR_INTERRUPTED
+    return code
+
+
+class InterruptToken:
+    """One runtime-interrupt flag (b2q_interrupt_token_*): pinned, device-mapped host memory that the running kernels poll.
+    `interrupt()` is a plain store, safe from any thread while a call runs; `reset()` is Executor::resetInterrupt."""
+
+    def __init__(self):
+        h = C.c_void_p()
+        rc = lib().b2q_interrupt_token_create(C.byref(h))
+        if rc:
+            _raise(rc)
+        self.h = h
+
+    def interrupt(self):
+        lib().b2q_interrupt(self.h)
+
+    def reset(self):
+        lib().b2q_interrupt_reset(self.h)
+
+    def is_set(self) -> bool:
+        return bool(lib().b2q_interrupt_is_set(self.h))
+
+    def __del__(self):
+        if getattr(self, "h", None):
+            lib().b2q_interrupt_token_destroy(self.h)
+            self.h = None
+
+
 def compilation_options(device_type: int = abi.DEVICE_GPU, hoist_literals: bool = True,
                         filter_on_deleted_column: bool = True) -> abi.CompilationOptions:
     """CompilationOptions::defaults(ExecutorDeviceType::GPU) — QueryEngine/CompilationOptions.h:52-65."""
@@ -194,9 +236,16 @@ def compilation_options(device_type: int = abi.DEVICE_GPU, hoist_literals: bool 
 
 
 def execution_options(allow_multifrag=True, output_columnar_hint=False, bigint_count=False, force_kernel=0,
-                      device_ordinal=-1, result_on_device=False) -> abi.ExecutionOptions:
+                      device_ordinal=-1, result_on_device=False, with_dynamic_watchdog=False, dynamic_watchdog_time_limit=10000,
+                      allow_runtime_query_interrupt=False, interrupt_token: Optional[InterruptToken] = None) -> abi.ExecutionOptions:
+    """ExecutionOptions (CompilationOptions.h:70-122).  dynamic_watchdog_time_limit is in ms (the reference's default 10 000,
+    Execute.cpp:87) and only counts with with_dynamic_watchdog; interrupt_token only with allow_runtime_query_interrupt."""
     eo = abi.ExecutionOptions()
     eo.result_on_device = int(result_on_device)
+    eo.with_dynamic_watchdog = int(with_dynamic_watchdog)
+    eo.dynamic_watchdog_time_limit = int(dynamic_watchdog_time_limit)
+    eo.allow_runtime_query_interrupt = int(allow_runtime_query_interrupt)
+    eo.interrupt_token = interrupt_token.h.value if interrupt_token is not None else None
     eo.allow_multifrag = int(allow_multifrag)
     eo.output_columnar_hint = int(output_columnar_hint)
     eo.bigint_count = int(bigint_count)
@@ -527,7 +576,29 @@ class Executor:
 
     def __init__(self, device_ordinal: int = -1):
         self.device_ordinal = device_ordinal
+        self._tokens = {}
         lib()
+
+    def interrupt_token(self, query_session: str) -> InterruptToken:
+        """The runtime-interrupt token of a session (made on first use).  A query of that session passes it in
+        execution_options(allow_runtime_query_interrupt=True, interrupt_token=...)."""
+        tok = self._tokens.get(query_session)
+        if tok is None:
+            tok = self._tokens[query_session] = InterruptToken()
+        return tok
+
+    def interrupt(self, query_session: str, interrupt_session: Optional[str] = None):
+        """Executor::interrupt(query_session, interrupt_session) (GpuInterrupt.cpp:33-160): stops the running (or next) call of
+        `query_session`, which then fails with ERR_INTERRUPTED.  `interrupt_session` names who asked (KILL QUERY's session);
+        it is not needed to find the query here."""
+        del interrupt_session
+        self.interrupt_token(query_session).interrupt()
+
+    def resetInterrupt(self, query_session: str):
+        """Executor::resetInterrupt (GpuInterrupt.cpp:292-300): the session's next query runs again."""
+        tok = self._tokens.get(query_session)
+        if tok is not None:
+            tok.reset()
 
     @staticmethod
     def _built_table(query_infos, memory_level):

@@ -37,7 +37,7 @@
 extern "C" {
 #endif
 
-#define B2Q_ABI_VERSION 8 /* 2: sort_info, join level, rte_idx, columnar, dictionary / time types, B2QPlan join fields;
+#define B2Q_ABI_VERSION 9 /* 2: sort_info, join level, rte_idx, columnar, dictionary / time types, B2QPlan join fields;
                             3: DATE_IN_DAYS chunks (negative col_encoded_sizes), column-vs-column quals, 16 filter leaves,
                                operands-before-node rule, b2q_columnar_results_*, host-phase stats;
                             4: DECIMAL / NUMERIC columns (B2QTypeInfo.scale), decimal_to_double of b2q_rs_get_next_row;
@@ -49,7 +49,9 @@ extern "C" {
                                B2Q_STAT_RESULT_D2H_BYTES;
                             7: projection units (B2Q_Projection: column targets, no GROUP BY, B2QExecUnit.scan_limit),
                                B2Q_STAT_ROWS_SCANNED, TOTAL_MATCHED / MAX_MATCHED of b2q_launch;
-                            8: B2Q_STAT_JOIN_TABLE (B2Q_JOIN_TABLE_*), b2q_last_launch_stat */
+                            8: B2Q_STAT_JOIN_TABLE (B2Q_JOIN_TABLE_*), b2q_last_launch_stat;
+                            9: B2QExecutionOptions.with_dynamic_watchdog / dynamic_watchdog_time_limit /
+                               allow_runtime_query_interrupt / interrupt_token, b2q_interrupt_token_* / b2q_interrupt[_reset] */
 
 /* ---- SQLTypes subset (Shared/sqltypes.h:65-99) -------------------------------------------------------- */
 enum {
@@ -277,7 +279,36 @@ typedef struct B2QExecutionOptions {
    * b2q_rs_device_columns reads the device copy directly.  0 = copy the result to the host before returning.  Planning is
    * the same either way; estimator results always come back to the host. */
   int32_t result_on_device;
+  /* Stopping a running call (ExecutionOptions::with_dynamic_watchdog / dynamic_watchdog_time_limit /
+   * allow_runtime_query_interrupt, CompilationOptions.h:80-81).  All zero = the call runs to its end, as before.
+   *   with_dynamic_watchdog: the call fails with B2Q_ERR_OUT_OF_TIME once its device work has run for
+   *     dynamic_watchdog_time_limit ms.  The budget covers ALL device work of one call, counted with %globaltimer from the
+   *     call's first kernel (the reference counts per kernel launch, in per-SM clock cycles, QueryExecutionContext.cpp:267).
+   *   allow_runtime_query_interrupt + interrupt_token: the call fails with B2Q_ERR_INTERRUPTED once b2q_interrupt(token) has
+   *     been called (before or during the call).  Interrupted + watchdog on + OUT_OF_TIME reports INTERRUPTED
+   *     (Execute.cpp:2319-2324).
+   * Long kernels (scan, radix partition / aggregate, projection) check between chunks: one lane per CTA reads %globaltimer per
+   * chunk and the token's flag at most every 100 us; the stop is cooperative (the kernel leaves its work loop, epilogues run,
+   * no trap).  The host also checks the token between host-resident slices, before a projection's second scan and between
+   * the host-synchronised steps of the device sort.  A stopped call returns no result set; its device memory is released
+   * stream-ordered and the next call on the same stream is unaffected.  b2q_launch does not check (it takes no options). */
+  int32_t with_dynamic_watchdog;
+  uint32_t dynamic_watchdog_time_limit;       /* ms */
+  int32_t allow_runtime_query_interrupt;
+  int32_t pad_;
+  const struct B2QInterruptToken* interrupt_token; /* NULL = none */
 } B2QExecutionOptions;
+
+/* ---- runtime query interrupt (Executor::interrupt / resetInterrupt, GpuInterrupt.cpp:33-160, :292-300) ----------------
+ * A token is one 32-bit flag in pinned, device-mapped, portable host memory: every device of a _multi call reads the same
+ * word.  b2q_interrupt is a plain store (no CUDA call, no stream): safe from any thread while a call runs.
+ * b2q_interrupt_reset clears the flag for the next query of the session.  Create without a CUDA device: B2Q_ERR_NO_DEVICE. */
+typedef struct B2QInterruptToken B2QInterruptToken;
+int32_t b2q_interrupt_token_create(B2QInterruptToken** out);
+void b2q_interrupt_token_destroy(B2QInterruptToken* token);
+void b2q_interrupt(B2QInterruptToken* token);
+void b2q_interrupt_reset(B2QInterruptToken* token);
+int32_t b2q_interrupt_is_set(const B2QInterruptToken* token); /* 1 after b2q_interrupt, 0 after create / reset */
 
 /* static kernel families (one per C symbol b2q_k_*) */
 enum {

@@ -16,6 +16,8 @@
 #pragma once
 #include <cstdint>
 #include <list>
+#include <map>
+#include <mutex>
 #include <optional>
 #include <memory>
 #include <stdexcept>
@@ -177,6 +179,11 @@ struct ExecutionOptions { /* CompilationOptions.h:70-122 */
   bool output_columnar_hint{false};
   bool bigint_count{false}; /* g_bigint_count */
   bool result_on_device{false}; /* keep the result in device memory (B2QExecutionOptions::result_on_device) */
+  bool with_dynamic_watchdog{false};
+  unsigned dynamic_watchdog_time_limit{10000}; /* ms (Execute.cpp:87) */
+  bool allow_runtime_query_interrupt{false};
+  /* the session's token (Executor::interruptToken): what Executor::interrupt(query_session, ...) sets */
+  const B2QInterruptToken* interrupt_token{nullptr};
   static ExecutionOptions defaults() { return ExecutionOptions{}; }
 };
 struct RenderInfo;              /* unused on this path */
@@ -307,6 +314,20 @@ class DeviceColumnarResults {
 
 class Executor {
  public:
+  Executor() = default;
+  Executor(const Executor&) = delete;
+  Executor& operator=(const Executor&) = delete;
+  ~Executor() { for (auto& kv : tokens_) b2q_interrupt_token_destroy(kv.second); }
+
+  /* the runtime-interrupt token of a session (made on first use); a query of the session passes it in
+   * ExecutionOptions::interrupt_token together with allow_runtime_query_interrupt */
+  const B2QInterruptToken* interruptToken(const std::string& query_session) { return token(query_session); }
+  /* Executor::interrupt(query_session, interrupt_session) (GpuInterrupt.cpp:33-160): the session's running (or next) call
+   * fails with B2Q_ERR_INTERRUPTED.  A plain store: safe from any thread while the call runs. */
+  void interrupt(const std::string& query_session, const std::string& /*interrupt_session*/) { b2q_interrupt(token(query_session)); }
+  /* Executor::resetInterrupt (GpuInterrupt.cpp:292-300) */
+  void resetInterrupt(const std::string& query_session) { b2q_interrupt_reset(token(query_session)); }
+
   ResultSetPtr executeWorkUnit(size_t& max_groups_buffer_entry_guess, const bool is_agg,
                                const std::vector<InputTableInfo>& query_infos, const RelAlgExecutionUnit& ra_exe_unit,
                                const CompilationOptions& co, const ExecutionOptions& options, RenderInfo* /*render_info*/,
@@ -399,7 +420,8 @@ class Executor {
     u.has_window_function = ra_exe_unit.has_window_function;
     B2QCompilationOptions cco{static_cast<int32_t>(co.device_type), co.hoist_literals ? 1 : 0, co.filter_on_deleted_column ? 0 : 1, 0};
     B2QExecutionOptions ceo{options.allow_multifrag ? 1 : 0, options.output_columnar_hint ? 1 : 0, options.bigint_count ? 1 : 0, 0, -1,
-                            options.result_on_device ? 1 : 0};
+                            options.result_on_device ? 1 : 0, options.with_dynamic_watchdog ? 1 : 0, options.dynamic_watchdog_time_limit,
+                            options.allow_runtime_query_interrupt ? 1 : 0, 0, options.interrupt_token};
     B2QResultSet* rs = nullptr;
     int32_t rc;
     if (storage) {
@@ -418,6 +440,19 @@ class Executor {
     }
     return std::make_shared<ResultSet>(rs);
   }
+
+  B2QInterruptToken* token(const std::string& session) {
+    std::lock_guard<std::mutex> g(tokens_mu_);
+    auto it = tokens_.find(session);
+    if (it != tokens_.end()) return it->second;
+    B2QInterruptToken* t = nullptr;
+    const int32_t rc = b2q_interrupt_token_create(&t);
+    if (rc != B2Q_OK) throw QueryExecutionError(rc, b2q_last_error_message());
+    tokens_.emplace(session, t);
+    return t;
+  }
+  std::mutex tokens_mu_;
+  std::map<std::string, B2QInterruptToken*> tokens_;
 };
 
 }  // namespace b2q
