@@ -12,6 +12,8 @@
 #include <stdint.h>
 #include <string.h>
 
+#include <vector>
+
 #include "../../include/b2q.h"
 
 #define B2Q_MAX_COLS 16   /* distinct columns a query may reference */
@@ -44,8 +46,12 @@ struct DevTerm {
   int8_t op2;           /* B2Q_kEQ .. B2Q_kGE */
   int32_t col2;         /* -1: comparison with a constant */
   int8_t nullable1, nullable2;
-  int8_t pad_[2];
+  /* set term (an IN / NOT IN list past the leaf program): in_range = v in [lo, lo + span] and bit v - lo of set_bits is set,
+   * tested on the register-class value like the range test; negate and null_check as above (a NULL row is never TRUE) */
+  int8_t is_set;
+  int8_t pad_;
   int64_t null_bits2;
+  const uint32_t* set_bits; /* device bitmap over [lo, lo + span], built per call from B2QQuery::set_values (executor.cpp) */
 };
 
 enum { FOP_TERM = 0, FOP_AND = 1, FOP_OR = 2 };
@@ -533,4 +539,7 @@ struct B2QQuery {
   int64_t limit, offset;
   int64_t total_tuples;          /* rows of all fragments of the table (every device's) */
   DevProject proj;               /* plan.query_desc_type == B2Q_Projection */
+  /* the values of set term t (prog.filter.terms[t].is_set): sorted, unique, in the column's register class (days for a
+   * days-encoded DATE); empty for every other term */
+  std::vector<int64_t> set_values[B2Q_MAX_TERMS];
 };

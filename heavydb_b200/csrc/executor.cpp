@@ -65,6 +65,8 @@ cudaError_t launch_project(const B2QQuery& q, const int8_t* const* col_ptrs, con
                            unsigned long long* counters, int32_t* error, const DevInterrupt& intr, cudaStream_t st);
 cudaError_t launch_watchdog_start(uint64_t* t0, cudaStream_t st);
 cudaError_t launch_set_error(int32_t* error, int32_t code, cudaStream_t st);
+size_t set_bytes(const B2QQuery& q);
+cudaError_t build_sets(B2QQuery& q, int8_t* blk, int* launches, cudaStream_t st);
 }  // namespace b2q
 
 using namespace b2q;
@@ -413,7 +415,7 @@ static int32_t alloc_partial(B2QPartial& p, size_t extra_bytes, cudaStream_t st)
   configure_pool_once(p.device);
   p.stream = st;
   const size_t n = std::max<size_t>(static_cast<size_t>(q.plan.entry_count), 1);
-  CU(p.blk.alloc(table_bytes(q) + DeviceBlock::pad(extra_bytes) + 4096, st));
+  CU(p.blk.alloc(table_bytes(q) + DeviceBlock::pad(extra_bytes) + DeviceBlock::pad(set_bytes(q)) + 4096, st));
   /* arrays of one reduction class (int64 SUM: COUNT / SUM_I64; f64 SUM; MIN; MAX; flags; bitmap) sit next to each other, so
    * that the cross-GPU merge is ONE collective per class over a contiguous range (C2: COUNT + SUM = one all-reduce) */
   for (int cls = 0; cls < kMergeClasses; ++cls)
@@ -423,6 +425,11 @@ static int32_t alloc_partial(B2QPartial& p, size_t extra_bytes, cudaStream_t st)
   if (q.smem.use_smem) p.smem_image = p.blk.take(std::max<int>(q.smem.replica_bytes, 16));
   p.d_error = reinterpret_cast<int32_t*>(p.blk.take(256));
   p.split = split_layout(q, p.radix);
+  if (const size_t sb = set_bytes(q)) { /* set terms: this device's own bitmaps, in the block, before the first scan */
+    int n = 0;
+    CU(build_sets(p.q, p.blk.take(sb), &n, st));
+    p.launches += n;
+  }
   for (auto& e : p.ev) CU(cudaEventCreate(&e));
   CU(cudaMemsetAsync(p.d_error, 0, sizeof(int32_t), st));
   CU(cudaEventRecord(p.ev[0], st));
@@ -1612,13 +1619,21 @@ static int32_t execute_projection_impl(const B2QTableInfo* tbl, const B2QExecUni
   } else if (u->scan_limit == 0) {
     rc = projection_count(tbl, u, co, eo, st, intr, &cap, &rs->h2d_bytes);
     if (rc != B2Q_OK) return rc;
-    rs->launches += 2;
+    rs->launches += set_bytes(q) ? 3 : 2; /* its b2q_k_init and scan, and its own set build */
     if (intr->interrupted()) return set_err(B2Q_ERR_INTERRUPTED, "the query was interrupted (b2q_interrupt on its token) after its row count");
   }
   projection_relayout(q, cap);
   const B2QPlan at_cap = q.plan;
   int8_t* d_out = nullptr;
-  CU(cudaMallocAsync(reinterpret_cast<void**>(&d_out), std::max<int64_t>(at_cap.buffer_size, 8), st));
+  /* the output buffer, followed by the bitmaps of the set terms */
+  const size_t out_bytes = DeviceBlock::pad(static_cast<size_t>(std::max<int64_t>(at_cap.buffer_size, 8)));
+  CU(cudaMallocAsync(reinterpret_cast<void**>(&d_out), out_bytes + set_bytes(q), st));
+  if (set_bytes(q) && !rows.empty() && cap) {
+    int n = 0;
+    const cudaError_t e = build_sets(q, d_out + out_bytes, &n, st);
+    if (e != cudaSuccess) { cudaGetLastError(); cudaFreeAsync(d_out, st); return set_err(B2Q_ERR_CUDA, std::string("IN-list bitmaps: ") + cudaGetErrorString(e)); }
+    rs->launches += n;
+  }
   ProjectRun run;
   if (tbl->memory_level == B2Q_CPU_LEVEL) rc = project_scan_host(q, cols, rows, d_out, cap, st, intr.get(), &run, &rs->h2d_bytes, &rs->host);
   else rc = project_scan(q, cols, rows, d_out, cap, st, intr->dev, &run);
@@ -1795,6 +1810,9 @@ void b2q_partial_free(B2QPartial* p) { delete p; }
  * device (params->group_by_buffers[0]) instead of returning a host ResultSet. */
 int32_t b2q_launch(const B2QQuery* query, const B2QParams* prm, void* stream) {
   if (!query || !prm) return set_err(B2Q_ERR_INVALID_ARGUMENT, "null argument");
+  if (set_bytes(*query))
+    return set_err(B2Q_ERR_UNSUPPORTED, "the filter holds an IN list planned as a value set, whose bitmap is built in memory of the call; "
+                                        "b2q_launch runs on caller memory only: use b2q_execute_work_unit / b2q_execute_partial");
   if (!have_device()) return set_err(B2Q_ERR_NO_DEVICE, "no CUDA device visible; this path has no CPU fallback");
   if (prm->row_func_mgr) return set_err(B2Q_ERR_UNSUPPORTED, "row function manager");
   if (query->plan.query_desc_type == B2Q_Estimator) return set_err(B2Q_ERR_UNSUPPORTED, "estimator queries run through b2q_execute_work_unit / b2q_execute_partial");

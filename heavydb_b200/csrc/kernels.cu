@@ -120,6 +120,26 @@ __global__ void b2q_k_bitmap_or(uint64_t* __restrict__ dst, const uint64_t* __re
   }
 }
 
+/* the bitmaps of a query's set terms (DevTerm::set_bits), zeroed beforehand: one atomicOr per value (InValuesBitmap's
+ * constructor, InValuesBitmap.cpp:40-95, done on the device).  values[i] belongs to the first set s with i < end[s]. */
+struct SetBuildArgs {
+  const int64_t* values;         /* every set's values, set after set */
+  uint32_t* bits[B2Q_MAX_TERMS];
+  int64_t end[B2Q_MAX_TERMS];    /* exclusive prefix ends into values */
+  int64_t min[B2Q_MAX_TERMS];
+  int32_t n_sets;
+};
+__global__ void b2q_k_set_build(const SetBuildArgs a) {
+  const int64_t n = a.end[a.n_sets - 1];
+  const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) {
+    int s = 0;
+    while (i >= a.end[s]) ++s;
+    const uint64_t d = (uint64_t)a.values[i] - (uint64_t)a.min[s];
+    atomicOr(a.bits[s] + (d >> 5), 1u << (uint32_t)(d & 31));
+  }
+}
+
 /* ---------------------------------------------------------------------------------------------------------
  * materialise: dense accumulators -> the reference's row-wise output buffer
  * (layout: QueryMemoryDescriptor.cpp:848-955; empty-entry conventions: ResultSetIteration.cpp:2457-2492)
@@ -386,6 +406,48 @@ cudaError_t launch_bitmap_or(uint64_t* dst, const uint64_t* gathered, int64_t wo
   int64_t blocks = (words + 255) / 256;
   if (blocks > cap) blocks = cap;
   b2q_k_bitmap_or<<<(int)blocks, 256, 0, st>>>(dst, gathered, words, copies);
+  return cudaGetLastError();
+}
+
+/* The set terms of `q` get their bitmaps in `blk` (set_bytes(q) bytes, device memory): the value lists are copied in after
+ * the bitmaps, the bitmaps zeroed and built by one kernel, and each term's set_bits points at its bitmap.  Returns the kernels
+ * launched (0 without a set term). */
+size_t set_bytes(const B2QQuery& q) {
+  size_t bytes = 0;
+  for (int t = 0; t < q.prog.filter.n_terms; ++t)
+    if (q.prog.filter.terms[t].is_set) bytes += ((q.prog.filter.terms[t].span >> 5) + 1) * 4 + q.set_values[t].size() * 8 + 16;
+  return bytes;
+}
+cudaError_t build_sets(B2QQuery& q, int8_t* blk, int* launches, cudaStream_t st) {
+  *launches = 0;
+  SetBuildArgs a;
+  memset(&a, 0, sizeof(a));
+  std::vector<int64_t> values;
+  size_t bits_bytes = 0;
+  for (int t = 0; t < q.prog.filter.n_terms; ++t) {
+    DevTerm& term = q.prog.filter.terms[t];
+    if (!term.is_set) continue;
+    const size_t words = (term.span >> 5) + 1;
+    term.set_bits = reinterpret_cast<const uint32_t*>(blk + bits_bytes);
+    a.bits[a.n_sets] = reinterpret_cast<uint32_t*>(blk + bits_bytes);
+    a.min[a.n_sets] = term.lo;
+    values.insert(values.end(), q.set_values[t].begin(), q.set_values[t].end());
+    a.end[a.n_sets++] = static_cast<int64_t>(values.size());
+    bits_bytes += (words * 4 + 15) & ~size_t(15);
+  }
+  if (!a.n_sets) return cudaSuccess;
+  int64_t* d_values = reinterpret_cast<int64_t*>(blk + bits_bytes);
+  a.values = d_values;
+  /* pageable source: the runtime has staged it when cudaMemcpyAsync returns */
+  cudaError_t e = cudaMemcpyAsync(d_values, values.data(), values.size() * 8, cudaMemcpyHostToDevice, st);
+  if (e == cudaSuccess) e = cudaMemsetAsync(blk, 0, bits_bytes, st);
+  if (e != cudaSuccess) return e;
+  const int block = 256;
+  int64_t blocks = (static_cast<int64_t>(values.size()) + block - 1) / block;
+  const int64_t cap = (int64_t)sm_count() * 8;
+  if (blocks > cap) blocks = cap;
+  b2q_k_set_build<<<(int)blocks, block, 0, st>>>(a);
+  *launches = 1;
   return cudaGetLastError();
 }
 

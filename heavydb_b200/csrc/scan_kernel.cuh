@@ -181,6 +181,13 @@ __device__ __forceinline__ void load32(int32_t (&v)[R], const int8_t* __restrict
   }
 }
 
+/* set term: a row in [lo, lo + span] is in the set when bit d = v - lo of the term's bitmap is set.  The bitmap is read through
+ * the read-only path with L1 allocation (the column stream bypasses L1), so a small bitmap stays in L1. */
+template <typename U>
+__device__ __forceinline__ bool set_bit(const uint32_t* __restrict__ bits, U d) {
+  return (__ldg(bits + (d >> 5)) >> (uint32_t)(d & 31)) & 1u;
+}
+
 /* ---------------------------------------------------------------------------------------------------------
  * filter: one comparison = one unsigned range test, (v - lo) <= span, in the column's register class
  * ------------------------------------------------------------------------------------------------------- */
@@ -195,7 +202,13 @@ __device__ __forceinline__ uint32_t eval_term(const DevTerm& t, const int8_t* co
       int64_t v[R];
       load64<!FULL>(v, cols[t.col], row0, stride, valid, pol, jidx, nullptr, jnull);
       const uint64_t lo = (uint64_t)t.lo, span = t.span;
-      if (lo == 0x8000000000000000ull) { /* only an upper bound (`<`, `<=`): one signed compare instead of subtract + compare */
+      if (t.is_set) {
+#pragma unroll
+        for (int j = 0; j < R; ++j) {
+          const uint64_t d = (uint64_t)v[j] - lo;
+          m |= (uint32_t)(((valid >> j & 1) && d <= span && set_bit(t.set_bits, d)) != neg) << j;
+        }
+      } else if (lo == 0x8000000000000000ull) { /* only an upper bound (`<`, `<=`): one signed compare instead of subtract + compare */
         const int64_t hi = (int64_t)(lo + span);
 #pragma unroll
         for (int j = 0; j < R; ++j) m |= (uint32_t)((v[j] <= hi) != neg) << j;
@@ -212,8 +225,16 @@ __device__ __forceinline__ uint32_t eval_term(const DevTerm& t, const int8_t* co
       int32_t v[R];
       load32<!FULL>(v, cols[t.col], t.width, row0, stride, valid, pol, jidx, jval, jnull);
       const uint32_t lo = (uint32_t)t.lo, span = (uint32_t)t.span;
+      if (t.is_set) {
 #pragma unroll
-      for (int j = 0; j < R; ++j) m |= (uint32_t)(((uint32_t)v[j] - lo <= span) != neg) << j;
+        for (int j = 0; j < R; ++j) {
+          const uint32_t d = (uint32_t)v[j] - lo;
+          m |= (uint32_t)(((valid >> j & 1) && d <= span && set_bit(t.set_bits, d)) != neg) << j;
+        }
+      } else {
+#pragma unroll
+        for (int j = 0; j < R; ++j) m |= (uint32_t)(((uint32_t)v[j] - lo <= span) != neg) << j;
+      }
       if (t.null_check) {
         const int32_t nullv = (int32_t)t.null_bits;
 #pragma unroll

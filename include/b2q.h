@@ -328,7 +328,8 @@ enum {
  * ======================================================================================================= */
 #define B2Q_MAX_SLOTS 16
 #define B2Q_MAX_TARGETS 16
-#define B2Q_MAX_FILTER_TERMS 16 /* comparison / IS NULL leaves of all quals together (an IN list is one leaf per value) */
+#define B2Q_MAX_FILTER_TERMS 16 /* comparison / IS NULL leaves of all quals together (an IN list is one leaf per value, consecutive
+                                   values one range; an integer IN / NOT IN list that does not fit is one term, a value set) */
 #define B2Q_MAX_GROUP_COLS 4
 
 typedef struct B2QTargetInfo { /* Shared/TargetInfo.h:49-78 */
