@@ -268,3 +268,21 @@ def test_module_rejects_wrong_special_values():
     g = fx.Group(np.array([-0.0, 0.0]), 2)
     assert fx.check_minmax(0.0, g, True, True) is None and fx.check_minmax(-0.0, g, False, True) is None
     assert fx.check_double_sum(None, fx.Group(np.zeros(0), 3)) is None
+
+
+@pytest.mark.parametrize("nullable", [True, False])
+@pytest.mark.parametrize("sql_type", [abi.kDOUBLE, abi.kFLOAT])
+def test_oracle_agrees_on_the_merge_special_values(sql_type, nullable):
+    """The groups test_gpu_multi_exact places across ranks (+-0 on two ranks, a NaN-only partial, +-inf, per-rank sums whose
+    total overflows), whole-table, against the same rules.  Left out for the reference only: group 22 in the nullable form,
+    whose first value is a NaN (the leading-NaN order dependence above), and the FLOAT group 30, which the reference adds in
+    float (2^24 + 1 rounds back to 2^24) where the product narrows its double sum once."""
+    import test_gpu_multi_exact as mx
+    null = fx.NULL_FLOAT if sql_type == abi.kFLOAT else fx.NULL_DOUBLE
+    spec = mx.fp_merge_groups(3, sql_type)
+    if not nullable:
+        spec = {key: {r: [1.0 if v == null else v for v in vals] for r, vals in pr.items()} for key, pr in spec.items()}
+    t, keys, vals = mx.rank_table(spec, 3, sql_type, not nullable, null, abi.NUMPY_OF[sql_type])
+    rows = oracle_lib.execute(sqlmini.parse(SPECIAL_SQL, t, ["k", "v"]), t, entry_guess=64, has_card=True).rows()
+    skip = ((22,) if nullable else ()) + ((30,) if sql_type == abi.kFLOAT else ())
+    assert check_special_rows(rows, keys, vals, sql_type, nullable, skip) == []

@@ -207,3 +207,56 @@ def test_result_set_sort_refuses_dictionary_string_targets():
             rs.sort(entries)
         ran += 1
     assert ran
+
+
+# ---- the datasets of the cross-device merge tests (test_gpu_multi_exact) ----------------------------------------------------------------
+def fragment_prefix_sums(groups, t, w, nullable, grouped):
+    """Record the running sums of fragments of unequal sizes (groups_of takes one fragment size), for SENTINEL_SUM."""
+    totals = {}
+    for f in t.fragments:
+        run = {}
+        for kk, x in zip(f.host_cols[0].tolist(), f.host_cols[1].tolist()):
+            g = kk if grouped else None
+            if nullable and x == w.null:
+                continue
+            run[g] = ix.wrap64(run.get(g, 0) + w.logical(x))
+            groups[g].prefix_sums.add(run[g])
+        for g, r in run.items():
+            totals[g] = ix.wrap64(totals.get(g, 0) + r)
+            groups[g].prefix_sums.add(totals[g])
+
+
+@pytest.mark.parametrize("nullable", [True, False])
+@pytest.mark.parametrize("k", [2, 3, 8])
+def test_oracle_equals_the_reference_on_the_merge_datasets(k, nullable):
+    """Groups that only a merge creates (per-rank SUMs that wrap while the total does not and the reverse, a group on one
+    rank only, NULL on one rank, MIN = MAX = INT64_MAX, values next to INT64_MIN) and the placement-edge table (skipped,
+    filtered-out and fully deleted fragments), over the whole table."""
+    import test_gpu_multi_exact as mx
+    w = ix.WIDTH["INT64"]
+    spec = mx.merge_edge_groups(k)
+    if not nullable:
+        spec = {key: {r: [1 if v is None else v for v in vals] for r, vals in pr.items()} for key, pr in spec.items()}
+    t, keys, phys = mx.rank_table(spec, k, abi.kBIGINT, not nullable, w.null, np.int64)
+    aggs = "COUNT(*), COUNT(v), SUM(v), MIN(v), MAX(v), AVG(v)"
+    for sql, ks in [(f"SELECT k, {aggs} FROM t GROUP BY k;", keys), (f"SELECT {aggs} FROM t;", None)]:
+        res = oracle_lib.execute(sqlmini.parse(sql, t, ["k", "v"]), t, entry_guess=64, has_card=True)
+        groups = ix.groups_of(w, ks, phys, nullable)
+        fragment_prefix_sums(groups, t, w, nullable, grouped=ks is not None)
+        bad, _skipped = check_rows(res.rows(decimal_to_double=False), res.plan, groups, w)
+        assert not bad, (sql, bad[:6])
+    t, keys, v, _d, m = mx.placement_table(k)
+    for sql, ks in [("SELECT k, COUNT(*), COUNT(v), SUM(v), MIN(v), MAX(v), AVG(v) FROM t WHERE k < 1000 AND (f > 0 OR f < 0) GROUP BY k;", keys),
+                    ("SELECT COUNT(*), COUNT(v), SUM(v), MIN(v), MAX(v), AVG(v) FROM t WHERE k < 1000 AND (f > 0 OR f < 0);", None)]:
+        res = oracle_lib.execute(sqlmini.parse(sql, t, ["k", "v", "d", "f", "del"]), t)
+        bad, _skipped = check_rows(res.rows(decimal_to_double=False), res.plan, ix.groups_of(w, ks, v, True, mask=m), w)
+        assert not bad, (sql, bad[:6])
+    t, (keys, v, _s, _b) = mx.baseline_table(k)
+    n_keys = len(set(keys.tolist()))
+    res = oracle_lib.execute(sqlmini.parse("SELECT k, COUNT(*), COUNT(v), SUM(v), MIN(v), MAX(v), AVG(v) FROM t GROUP BY k;", t,
+                                           ["k", "v", "s", "b"]), t, entry_guess=2 * n_keys, has_card=True)
+    assert res.plan.query_desc_type == abi.GroupByBaselineHash
+    groups = ix.groups_of(w, keys, v, True, frag_rows=mx.BASELINE_FRAG)
+    groups = {None if kk == abi.NULL_BIGINT else kk: g for kk, g in groups.items()}
+    bad, _skipped = check_rows(res.rows(decimal_to_double=False), res.plan, groups, w)
+    assert not bad, bad[:6]

@@ -5,7 +5,8 @@ with SUM / MIN / MAX — checked against the oracle's own host reduce over all f
 
 The dense-array model below mirrors the decomposition the CUDA library uses for its accumulators
 (heavydb_b200/csrc/planner.cpp `lower`): COUNT and SUM as sums from 0, a non-NULL count next to every nullable
-SUM/MIN/MAX (it decides the NULL sentinel at materialisation), MIN/MAX from +-identity, doubles as they are.
+SUM/MIN/MAX (it decides the NULL sentinel at materialisation), MIN/MAX from +-identity, doubles as they are.  A merged
+MIN / MAX equal to its identity (+inf, INT64_MAX) is a value, not NULL: EDGE_QUERIES hold such groups.
 """
 import os
 import socket
@@ -30,6 +31,21 @@ QUERIES = [
     "SELECT COUNT(*), SUM(t), MIN(z), MAX(w), AVG(y), SUM(u) FROM test WHERE z > 0;",
     "SELECT t, SUM(x) FROM test GROUP BY t;",
 ]
+# over edge_table(): one row per fragment, so that both ranks hold part of every group
+EDGE_QUERIES = ["SELECT k, MIN(d), MAX(d), MIN(b), MAX(b), COUNT(d), COUNT(b) FROM e GROUP BY k;",
+                "SELECT MIN(d), MAX(d), MIN(b), MAX(b) FROM e WHERE k = 0;"]
+EDGE_NAMES = ["k", "d", "b"]
+
+
+def edge_table():
+    """Group 0: MIN(d) = +inf and MIN(b) = MAX(b) = INT64_MAX, the MIN identities; 1: -inf and INT64_MIN + 1; 2: a NULL
+    and a value on different ranks; 3: NULL only."""
+    inf, nd, nb = np.inf, abi.NULL_DOUBLE, abi.NULL_BIGINT
+    rows = [(0, inf, I64_MAX), (0, inf, I64_MAX), (1, -inf, I64_MIN + 1), (1, 5.0, 3), (2, 1.0, nb), (2, nd, 7), (3, nd, nb), (3, nd, nb)]
+    t = abi.Table([(abi.kINT, True), (abi.kDOUBLE, False), (abi.kBIGINT, False)])
+    for k, d, b in rows:
+        t.add_host_fragment([np.array([k], np.int32), np.array([d]), np.array([b], np.int64)])
+    return t
 
 
 def test_fragment_placement_rule():
@@ -83,8 +99,11 @@ def dense_arrays(res):
                 arrays.append((f"sum{ti}", w, abi.RED_SUM))
             arrays.append((f"nn{ti}", (~is_null & (touched > 0)).astype(np.int64) if t.agg_kind == abi.kSUM else slots[s + 1].copy(), abi.RED_SUM))
         else:
+            # MIN / MAX from +-identity, NULL decided by a non-NULL count (a real +inf or INT64_MAX is a value)
             ident = I64_MAX if t.agg_kind == abi.kMIN else I64_MIN
-            empty = (v == init) | (touched == 0)
+            nn = (touched > 0) & (v != init) if t.skip_null_val else touched > 0
+            empty = ~nn
+            arrays.append((f"nn{ti}", nn.astype(np.int64), abi.RED_SUM))
             if fp:
                 d = v.view(np.float64).copy()
                 d[empty] = np.inf if t.agg_kind == abi.kMIN else -np.inf
@@ -117,10 +136,23 @@ def rebuild_rows(plan, merged, key_of_entry):
                 row.append(None if c == 0 else float(m[f"sum{ti}"][i]) / c)
             else:
                 v = m[f"mm{ti}"][i]
-                null = (np.isinf(v) if fp else v in (I64_MAX, I64_MIN))
+                null = t.skip_null_val and m[f"nn{ti}"][i] == 0
                 row.append(None if null else (float(v) if fp else int(v)))
         rows.append(tuple(row))
     return rows
+
+
+def _placed(table, rank, world):
+    """This rank's fragments, the others as placeholders that carry only their chunk stats: chunk stats drive the plan
+    (entry_count, keyless...), so every rank must plan on the WHOLE table's stats, exactly like the reference plans once for
+    all devices."""
+    plan_table = abi.Table(table.col_types)
+    for fid, f in enumerate(table.fragments):
+        if fid % world == rank:
+            plan_table.fragments.append(f)
+        else:
+            plan_table.fragments.append(abi.Fragment(0, host_cols=[None] * len(f.host_cols), stats=f.stats, fragment_id=fid))
+    return plan_table
 
 
 def _worker(rank, world, port, out_q):
@@ -128,24 +160,13 @@ def _worker(rank, world, port, out_q):
     os.environ["MASTER_PORT"] = str(port)
     dist.init_process_group("gloo", rank=rank, world_size=world)
     try:
-        rows = rt.test_rows()
-        full = rt.make_table(rows)                      # 10 fragments of 2 rows
-        mine = abi.Table(full.col_types)
-        for fid in multigpu.shard_fragments(range(len(full.fragments)), rank, world):
-            mine.fragments.append(full.fragments[fid])
-        # chunk stats drive the plan (entry_count, keyless...): every rank must plan on the WHOLE table's stats,
-        # exactly like the reference plans once for all devices.  Carry empty-fragment placeholders with the stats.
-        plan_table = abi.Table(full.col_types)
-        for fid, f in enumerate(full.fragments):
-            if fid % world == rank:
-                plan_table.fragments.append(f)
-            else:
-                plan_table.fragments.append(abi.Fragment(0, host_cols=[None] * len(f.host_cols), stats=f.stats, fragment_id=fid))
+        full = rt.make_table(rt.test_rows())                      # 10 fragments of 2 rows
         ok = True
-        for sql in QUERIES:
-            unit = sqlmini.parse(sql, full, rt.TEST_NAMES)
+        for sql, names, table in [(q, rt.TEST_NAMES, full) for q in QUERIES] + [(q, EDGE_NAMES, edge_table()) for q in EDGE_QUERIES]:
+            plan_table = _placed(table, rank, world)
+            unit = sqlmini.parse(sql, table, names)
             local = oracle_lib.execute(unit, plan_table)
-            want = oracle_lib.execute(unit, full)
+            want = oracle_lib.execute(unit, table)
             assert local.plan.as_dict() == want.plan.as_dict()
             arrays = dense_arrays(local)
             tensors = [(torch.from_numpy(a), op) for _, a, op in arrays]
@@ -163,6 +184,7 @@ def _worker(rank, world, port, out_q):
                 ok = False
                 out_q.put((rank, sql, str(e)[:500]))
         # the estimator query: per-rank linear-counting bitmaps merge with OR (reduce_estimator_results)
+        plan_table = _placed(full, rank, world)
         for cols in (["t"], ["x", "y"]):
             b = abi.UnitBuilder(full)
             b.estimator([rt.TEST_NAMES.index(c) for c in cols])
