@@ -530,7 +530,9 @@ class BuiltUnit:
         self.inner = b.inner
         if b.inner is not None:
             assert len(b.inner.fragments) <= 1, "the inner table must be one concatenated fragment"
-            self._inner_built = b.inner.build(CPU_LEVEL)     # host chunks; the library copies what it needs
+            # host chunks (the library copies what it needs), or the device columns of a temporary table
+            device = any(f.dev_ptrs for f in b.inner.fragments)
+            self._inner_built = b.inner.build(GPU_LEVEL if device else CPU_LEVEL)
             u.num_join_quals, u.join_qual, u.join_type = 1, b.join_qual, b.join_type
             u.inner_table = C.cast(C.pointer(self._inner_built.info), C.c_void_p)
         for k, v in b.unsupported.items():
@@ -592,6 +594,7 @@ class Table:
         self.deleted_column = deleted_column
         self.col_scales: Dict[int, int] = dict(col_scales or {})   # DECIMAL / NUMERIC columns: column index -> scale
         self.fragments: List[Fragment] = []
+        self.owner = None   # what owns the device memory of device fragments (a temporary table's DeviceColumns)
 
     def physical_dtype(self, c: int):
         """numpy dtype of the chunk elements of column c (narrower than the logical type under ENCODING FIXED)."""

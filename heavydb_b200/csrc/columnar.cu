@@ -10,12 +10,17 @@
  *   2. one conversion kernel: thread r decodes row r with the host reader's own per-slot code (b2q_read_target,
  *      b2q_internal.h), writes every target at its width, an Arrow validity word per 32 rows (__ballot_sync) and, for
  *      DECIMAL targets, the decimal128 image Arrow wants.  The buffer is read once and every column written once.
+ *      The same pass keeps each column's chunk stats (synthesize_metadata, InputMetadata.cpp:381-470): every value is
+ *      mapped to an order-preserving unsigned key, a warp takes the min / max key with __reduce_max_sync, a CTA with a
+ *      shared-memory atomic and the grid with one global atomic per column; the keys ride the NULL-count copy back.
  */
 #include <cuda_runtime.h>
 
 #include <algorithm>
 #include <atomic>
+#include <cfloat>
 #include <cstdio>
+#include <cstring>
 #include <string>
 #include <vector>
 
@@ -41,18 +46,49 @@ struct DevColumnsOut {
   int8_t* dec128[B2Q_MAX_TARGETS]; /* DECIMAL targets: 16 bytes per row, the int64 sign-extended; else nullptr */
   int64_t null_bits[B2Q_MAX_TARGETS];
   int8_t width[B2Q_MAX_TARGETS];
+  int8_t is_fp[B2Q_MAX_TARGETS];
   int32_t n_cols;
 };
 
 constexpr int COL_BLOCK = 256;
+constexpr uint64_t SIGN64 = 0x8000000000000000ull;
+
+/* Order-preserving keys of a stored value (bits as b2q_store_target returns them): signed integers with the sign bit
+ * flipped, IEEE floats with every bit flipped when negative and the sign bit flipped otherwise (-0 sorts below +0).
+ * Columns of 4 bytes or less use 32-bit keys, 8-byte columns 64-bit ones. */
+__host__ __device__ inline uint32_t key32(int64_t bits, bool fp) {
+  const uint32_t b = static_cast<uint32_t>(bits);
+  return fp && (b >> 31) ? ~b : b ^ 0x80000000u;
+}
+__host__ __device__ inline uint64_t key64(int64_t bits, bool fp) {
+  const uint64_t b = static_cast<uint64_t>(bits);
+  return fp && (b >> 63) ? ~b : b ^ SIGN64;
+}
+
+/* the largest key of the warp; the 64-bit one as its high word, then the low word among the lanes that hold that high word */
+__device__ inline uint64_t warp_max_key(uint64_t k, bool wide) {
+  if (!wide) return __reduce_max_sync(~0u, static_cast<uint32_t>(k));
+  const uint32_t hi = __reduce_max_sync(~0u, static_cast<uint32_t>(k >> 32));
+  const uint32_t lo = __reduce_max_sync(~0u, static_cast<uint32_t>(k >> 32) == hi ? static_cast<uint32_t>(k) : 0u);
+  return (static_cast<uint64_t>(hi) << 32) | lo;
+}
 
 /* row r of the output = entry entries[first + r] (or first + r when every entry is visited in order) */
 __global__ void __launch_bounds__(COL_BLOCK) b2q_k_device_columns(const __grid_constant__ B2QPlan p, const int8_t* __restrict__ buf,
                                                                  const uint32_t* __restrict__ entries, int64_t first, int64_t n,
                                                                  const __grid_constant__ DevColumnsOut o,
                                                                  unsigned long long* __restrict__ null_counts) {
+  /* null_counts[c]; then per column the complement of its smallest key and its largest key, both 0 when no value
+   * entered the range (a NULL or a NaN never does) */
+  unsigned long long* const neg_min_keys = null_counts + B2Q_MAX_TARGETS;
+  unsigned long long* const max_keys = null_counts + 2 * B2Q_MAX_TARGETS;
   __shared__ unsigned int s_nulls[B2Q_MAX_TARGETS];
-  if (threadIdx.x < B2Q_MAX_TARGETS) s_nulls[threadIdx.x] = 0;
+  __shared__ unsigned long long s_neg_min[B2Q_MAX_TARGETS], s_max[B2Q_MAX_TARGETS];
+  if (threadIdx.x < B2Q_MAX_TARGETS) {
+    s_nulls[threadIdx.x] = 0;
+    s_neg_min[threadIdx.x] = 0;
+    s_max[threadIdx.x] = 0;
+  }
   __syncthreads();
   const int lane = threadIdx.x & 31;
   const int64_t stride = (int64_t)gridDim.x * blockDim.x;
@@ -63,6 +99,8 @@ __global__ void __launch_bounds__(COL_BLOCK) b2q_k_device_columns(const __grid_c
     const unsigned in_mask = __ballot_sync(~0u, in);
     for (int c = 0; c < o.n_cols; ++c) {
       bool valid = false;
+      const bool wide = o.width[c] == 8;
+      uint64_t neg_min = 0, mx = 0;
       if (in) {
         B2QTargetValue v;
         b2q_read_target(p, buf, e, c, false, &v); /* decimals stay scaled int64, as in ColumnarResults */
@@ -74,17 +112,63 @@ __global__ void __launch_bounds__(COL_BLOCK) b2q_k_device_columns(const __grid_c
           d[0] = bits;
           d[1] = bits >> 63;
         }
+        /* NoneEncoder::updateStats: std::min / std::max never take a NaN */
+        const bool nan = o.is_fp[c] && (wide ? (static_cast<uint64_t>(bits) << 1) > (0x7FF0000000000000ull << 1)
+                                             : (static_cast<uint32_t>(bits) << 1) > (0x7F800000u << 1));
+        if (valid && !nan) {
+          mx = wide ? key64(bits, o.is_fp[c]) : key32(bits, o.is_fp[c]);
+          neg_min = wide ? ~mx : ~static_cast<uint32_t>(mx);
+        }
       }
       const unsigned vm = __ballot_sync(~0u, valid);
+      neg_min = warp_max_key(neg_min, wide);
+      mx = warp_max_key(mx, wide);
       if (lane == 0) {
         o.validity[c][r >> 5] = vm;
         const unsigned nulls = __popc(in_mask & ~vm);
         if (nulls) atomicAdd(&s_nulls[c], nulls);
+        if (neg_min) atomicMax(&s_neg_min[c], (unsigned long long)neg_min);
+        if (mx) atomicMax(&s_max[c], (unsigned long long)mx);
       }
     }
   }
   __syncthreads();
-  if (threadIdx.x < o.n_cols && s_nulls[threadIdx.x]) atomicAdd(&null_counts[threadIdx.x], (unsigned long long)s_nulls[threadIdx.x]);
+  if (threadIdx.x < o.n_cols) {
+    const int c = threadIdx.x;
+    if (s_nulls[c]) atomicAdd(&null_counts[c], (unsigned long long)s_nulls[c]);
+    if (s_neg_min[c]) atomicMax(&neg_min_keys[c], s_neg_min[c]);
+    if (s_max[c]) atomicMax(&max_keys[c], s_max[c]);
+  }
+}
+
+/* synthesize_metadata of one column from its reduced keys: a fresh NoneEncoder<T>'s stats (min = numeric_limits<T>::max(),
+ * max = lowest()) where no value entered the range.  A key of 0 never belongs to a value except the smallest key's
+ * complement of INT32_MAX / INT64_MAX, which then decodes to that same limit. */
+B2QChunkStats chunk_stats_from_keys(const B2QTypeInfo& ti, uint64_t neg_min, uint64_t max_key, int64_t null_count) {
+  B2QChunkStats s;
+  memset(&s, 0, sizeof(s));
+  s.has_nulls = null_count > 0;
+  const int t = ti.type;
+  if (t == B2Q_kDOUBLE || t == B2Q_kFLOAT) {
+    auto fp = [&](uint64_t k) {
+      if (t == B2Q_kDOUBLE) { const uint64_t b = (k >> 63) ? k ^ SIGN64 : ~k; double d; memcpy(&d, &b, 8); return d; }
+      const uint32_t k32 = static_cast<uint32_t>(k), b = (k32 >> 31) ? k32 ^ 0x80000000u : ~k32;
+      float f; memcpy(&f, &b, 4);
+      return static_cast<double>(f);
+    };
+    const double lim = t == B2Q_kDOUBLE ? DBL_MAX : static_cast<double>(FLT_MAX);
+    s.fp_min = neg_min ? fp(t == B2Q_kDOUBLE ? ~neg_min : static_cast<uint32_t>(~neg_min)) : lim;
+    s.fp_max = max_key ? fp(max_key) : -lim;
+    return s;
+  }
+  const int w = b2q_type_size(t);
+  const int64_t hi = w == 1 ? INT8_MAX : w == 2 ? INT16_MAX : w == 4 ? INT32_MAX : INT64_MAX;
+  auto val = [&](uint64_t k) {
+    return w == 8 ? static_cast<int64_t>(k ^ SIGN64) : static_cast<int64_t>(static_cast<int32_t>(static_cast<uint32_t>(k) ^ 0x80000000u));
+  };
+  s.int_min = neg_min ? val(w == 8 ? ~neg_min : static_cast<uint32_t>(~neg_min)) : hi;
+  s.int_max = max_key ? val(max_key) : -hi - 1;
+  return s;
 }
 
 size_t pad256(size_t n) { return (n + 255) & ~size_t(255); }
@@ -129,6 +213,7 @@ struct B2QDeviceColumns {
   uint32_t* validity[B2Q_MAX_TARGETS];
   int8_t* dec128[B2Q_MAX_TARGETS];
   int64_t null_count[B2Q_MAX_TARGETS];
+  B2QChunkStats stats[B2Q_MAX_TARGETS];
 };
 
 namespace {
@@ -253,7 +338,8 @@ int32_t b2q_rs_device_columns(const B2QResultSet* rs, void* stream, B2QDeviceCol
   dc->n = n;
   /* 2. one allocation for every output buffer */
   const size_t words = (std::max<size_t>(n, 1) + 31) / 32;
-  size_t bytes = pad256(static_cast<size_t>(B2Q_MAX_TARGETS) * 8);
+  const size_t counters = static_cast<size_t>(B2Q_MAX_TARGETS) * 3 * 8; /* NULL counts, smallest-key complements, largest keys */
+  size_t bytes = pad256(counters);
   for (int c = 0; c < nt; ++c) {
     dc->types[c] = b2q_target_col_type(p.targets[c]);
     dc->width[c] = b2q_type_size(dc->types[c].type);
@@ -264,7 +350,7 @@ int32_t b2q_rs_device_columns(const B2QResultSet* rs, void* stream, B2QDeviceCol
   if (e != cudaSuccess) { sh->base = nullptr; return fail(B2Q_ERR_OUT_OF_GPU_MEM, "device columns"); }
   int8_t* q = sh->base;
   unsigned long long* d_nulls = reinterpret_cast<unsigned long long*>(q);
-  q += pad256(static_cast<size_t>(B2Q_MAX_TARGETS) * 8);
+  q += pad256(counters);
   DevColumnsOut o;
   memset(&o, 0, sizeof(o));
   o.n_cols = nt;
@@ -278,9 +364,10 @@ int32_t b2q_rs_device_columns(const B2QResultSet* rs, void* stream, B2QDeviceCol
     o.dec128[c] = dc->dec128[c];
     o.width[c] = static_cast<int8_t>(dc->width[c]);
     o.null_bits[c] = b2q_null_bits(dc->types[c].type);
+    o.is_fp[c] = dc->types[c].type == B2Q_kDOUBLE || dc->types[c].type == B2Q_kFLOAT;
   }
   if (cudaEventCreate(&ev0) != cudaSuccess || cudaEventCreate(&sh->done) != cudaSuccess) return fail(B2Q_ERR_CUDA, "cudaEventCreate");
-  e = cudaMemsetAsync(d_nulls, 0, static_cast<size_t>(B2Q_MAX_TARGETS) * 8, st);
+  e = cudaMemsetAsync(d_nulls, 0, counters, st);
   if (e == cudaSuccess) e = cudaEventRecord(ev0, st);
   if (e == cudaSuccess && n > 0 && nt > 0) {
     const int64_t blocks = std::min<int64_t>((static_cast<int64_t>(n) + COL_BLOCK - 1) / COL_BLOCK, static_cast<int64_t>(sm_count()) * 16);
@@ -289,8 +376,8 @@ int32_t b2q_rs_device_columns(const B2QResultSet* rs, void* stream, B2QDeviceCol
     e = cudaGetLastError();
   }
   if (e == cudaSuccess) e = cudaEventRecord(sh->done, st);
-  unsigned long long h_nulls[B2Q_MAX_TARGETS] = {};
-  if (e == cudaSuccess) e = cudaMemcpyAsync(h_nulls, d_nulls, static_cast<size_t>(B2Q_MAX_TARGETS) * 8, cudaMemcpyDeviceToHost, st);
+  unsigned long long h_nulls[3 * B2Q_MAX_TARGETS] = {};
+  if (e == cudaSuccess) e = cudaMemcpyAsync(h_nulls, d_nulls, counters, cudaMemcpyDeviceToHost, st);
   for (void* t : temps) cudaFreeAsync(t, st);
   temps.clear();
   if (e == cudaSuccess) e = cudaStreamSynchronize(st);
@@ -298,7 +385,10 @@ int32_t b2q_rs_device_columns(const B2QResultSet* rs, void* stream, B2QDeviceCol
   float ms = 0;
   if (cudaEventElapsedTime(&ms, ev0, sh->done) == cudaSuccess) dc->convert_ms = ms;
   cudaEventDestroy(ev0);
-  for (int c = 0; c < nt; ++c) dc->null_count[c] = static_cast<int64_t>(h_nulls[c]);
+  for (int c = 0; c < nt; ++c) {
+    dc->null_count[c] = static_cast<int64_t>(h_nulls[c]);
+    dc->stats[c] = chunk_stats_from_keys(dc->types[c], h_nulls[B2Q_MAX_TARGETS + c], h_nulls[2 * B2Q_MAX_TARGETS + c], dc->null_count[c]);
+  }
   if (caller >= 0 && caller != device) cudaSetDevice(caller);
   cudaGetLastError();
   *out = dc;
@@ -316,6 +406,12 @@ const void* b2q_device_columns_column(const B2QDeviceColumns* dc, size_t col, B2
   if (validity) *validity = dc->null_count[col] ? dc->validity[col] : nullptr;
   if (null_count) *null_count = dc->null_count[col];
   return dc->values[col];
+}
+
+int32_t b2q_device_columns_chunk_stats(const B2QDeviceColumns* dc, size_t col, B2QChunkStats* out) {
+  if (!dc || !out || col >= static_cast<size_t>(dc->nt)) return report_error(B2Q_ERR_INVALID_ARGUMENT, "no such device column");
+  *out = dc->stats[col];
+  return B2Q_OK;
 }
 
 int32_t b2q_device_columns_export_arrow(B2QDeviceColumns* dc, const char* const* names, ArrowSchema* schema, ArrowDeviceArray* array) {

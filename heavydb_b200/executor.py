@@ -170,6 +170,8 @@ def lib():
         L.b2q_device_columns_export_arrow.argtypes = [C.c_void_p, C.POINTER(C.c_char_p), C.POINTER(abi.ArrowSchema),
                                                       C.POINTER(abi.ArrowDeviceArray)]
         L.b2q_device_columns_free.argtypes = [C.c_void_p, C.c_void_p]
+        L.b2q_device_columns_chunk_stats.restype = C.c_int32
+        L.b2q_device_columns_chunk_stats.argtypes = [C.c_void_p, C.c_size_t, C.POINTER(abi.ChunkStats)]
         L.b2q_interrupt_token_create.restype = C.c_int32
         L.b2q_interrupt_token_create.argtypes = [C.POINTER(C.c_void_p)]
         for n in ("b2q_interrupt_token_destroy", "b2q_interrupt", "b2q_interrupt_reset"):
@@ -514,6 +516,33 @@ class DeviceColumns:
             _p, (ty, nn, _sc), _v, nulls = self.column(i)
             out.append((ty, nn, vals.cpu().numpy(), None if mask is None else mask.cpu().numpy(), nulls))
         return out
+
+    def chunk_stats(self, i: int) -> abi.ChunkStats:
+        """synthesize_metadata (InputMetadata.cpp:381-470) of column i, computed by the conversion kernel
+        (b2q_device_columns_chunk_stats)."""
+        st = abi.ChunkStats()
+        rc = lib().b2q_device_columns_chunk_stats(self._h, i, C.byref(st))
+        if rc:
+            _raise(rc)
+        return st
+
+    def as_table(self) -> abi.Table:
+        """The temporary table the next step reads (ColumnFetcher::getResultSetColumn + synthesize_metadata): one
+        GPU_LEVEL fragment, fragment_id 0, on this object's device, over these columns and their chunk stats.  Run it with
+        memory_level=abi.GPU_LEVEL on that device.  The table holds a reference to this object, so the buffers outlive every
+        step that reads it."""
+        types, ptrs, scales = [], [], {}
+        for i in range(self.num_columns()):
+            ptr, (ty, nn, scale), _valid, _nulls = self.column(i)
+            types.append((ty, nn))
+            ptrs.append(ptr)
+            if scale:
+                scales[i] = scale
+        t = abi.Table(types, col_scales=scales)
+        t.add_device_fragment(self.size(), ptrs, [self.chunk_stats(i) for i in range(len(types))], fragment_id=0,
+                              device_id=self.device())
+        t.owner = self
+        return t
 
     def export_arrow(self, names=None) -> ArrowExport:
         """b2q_device_columns_export_arrow: the columns as an Arrow C Device record batch (a "+s" struct of one child per

@@ -308,3 +308,222 @@ def parse(sql: str, table: abi.Table, names: List[str], bigint_count: bool = Fal
     if not aggregate and p.b.estimator_kind == 0 and not p.b.order and p.b.limit is not None:
         p.b.scan_limit = p.b.limit + p.b.offset
     return p.b.build()
+
+
+# ---- work units of a multi-step query ------------------------------------------------------------------------------------
+_CLAUSES = ("FROM", "WHERE", "GROUP", "HAVING", "ORDER", "LIMIT", "OFFSET")
+_KEYWORDS = set(_CLAUSES) | {"SELECT", "JOIN", "LEFT", "INNER", "ON", "AS", "BY"}
+
+
+class Step:
+    """One work unit of parse_steps: `sql` is a query parse() accepts over its input tables.  `source` / `inner` name them:
+    a base table name (a str) or the index of an earlier step whose result is read as a temporary table; `inner` is None
+    without a join.  `names` are the step's output column names (the temporary table's column names)."""
+
+    def __init__(self, sql: str, source, inner, names: List[str]):
+        self.sql, self.source, self.inner, self.names = sql, source, inner, names
+
+    def __repr__(self):
+        return f"Step({self.sql!r}, source={self.source!r}, inner={self.inner!r}, names={self.names})"
+
+
+def _split_clauses(toks: List[str]):
+    """{clause: tokens} of one SELECT, split at parenthesis depth 0 (GROUP / ORDER without their BY)."""
+    out, cur, depth = {"SELECT": []}, "SELECT", 0
+    for i, tok in enumerate(toks[1:], 1):
+        up = tok.upper()
+        if depth == 0 and up in _CLAUSES:
+            cur = up
+            out[cur] = []
+            continue
+        if depth == 0 and up == "BY" and cur in ("GROUP", "ORDER") and not out[cur]:
+            continue
+        depth += tok == "("
+        depth -= tok == ")"
+        out[cur].append(tok)
+    return out
+
+
+def _split_commas(toks: List[str]) -> List[List[str]]:
+    parts, cur, depth = [], [], 0
+    for tok in toks:
+        if tok == "," and depth == 0:
+            parts.append(cur)
+            cur = []
+            continue
+        depth += tok == "("
+        depth -= tok == ")"
+        cur.append(tok)
+    return parts + [cur] if cur else parts
+
+
+def _is_agg(toks: List[str], j: int) -> bool:
+    return toks[j].upper() in _AGGS and j + 1 < len(toks) and toks[j + 1] == "("
+
+
+def _agg_text(toks: List[str], j: int):
+    """(canonical text, index after) of the aggregate call at toks[j] — the text parse()'s ORDER BY matching uses."""
+    k = toks.index(")", j)
+    return "".join(toks[j:k + 1]).upper(), k + 1
+
+
+def _output_names(select: List[List[str]]) -> List[str]:
+    """Column names of a SELECT list: the alias, else a column's own name, else EXPR<i> (Calcite's EXPR$<i>)."""
+    names = []
+    for i, t in enumerate(select):
+        if len(t) >= 2 and re.fullmatch(r"[A-Za-z_][A-Za-z_0-9]*", t[-1]) and (t[-2].upper() == "AS" or t[-2] == ")" or len(t) == 2):
+            names.append(t[-1].lower())
+        elif len(t) == 1:
+            names.append(t[0].split(".")[-1].lower())
+        else:
+            names.append(f"expr{i}")
+    return names
+
+
+def _source(toks: List[str], j: int, steps: List[Step], tables):
+    """A FROM item at toks[j]: a table name or a parenthesised SELECT, then an optional [AS] alias.  Returns (source, the
+    name the step's SQL uses for it, its column names, index after)."""
+    if toks[j] == "(":
+        depth, k = 0, j
+        while True:
+            depth += toks[k] == "("
+            depth -= toks[k] == ")"
+            if depth == 0:
+                break
+            k += 1
+        src = _plan(toks[j + 1:k], steps, tables)
+        j = k + 1
+        default = f"tmp{src}"
+        names = steps[src].names
+    else:
+        src = toks[j].lower()
+        default = src
+        names = tables[src][1] if src in tables else None
+        j += 1
+    if j < len(toks) and toks[j].upper() == "AS":
+        j += 1
+    alias = None
+    if j < len(toks) and toks[j].upper() not in _KEYWORDS and re.fullmatch(r"[A-Za-z_][A-Za-z_0-9]*", toks[j]):
+        alias = toks[j].lower()
+        j += 1
+    return src, alias or default, names, j
+
+
+def _plan(toks: List[str], steps: List[Step], tables) -> int:
+    """Append the steps of one SELECT (its subqueries first) and return the index of the step that yields its rows."""
+    if not toks or toks[0].upper() != "SELECT":
+        raise ValueError("a step must be a SELECT")
+    cl = _split_clauses(toks)
+    frm = cl.get("FROM")
+    if not frm:
+        raise ValueError("SELECT without FROM")
+    src, sname, _names, j = _source(frm, 0, steps, tables)
+    from_sql, inner = [sname], None
+    if j < len(frm):
+        if frm[j].upper() == "LEFT":
+            from_sql.append("LEFT")
+            j += 1
+        if frm[j].upper() == "INNER":
+            j += 1
+        if frm[j].upper() != "JOIN":
+            raise ValueError(f"unexpected {frm[j]} in FROM")
+        inner, iname, _inames, j = _source(frm, j + 1, steps, tables)
+        from_sql += ["JOIN", iname] + frm[j:]
+    select = _split_commas(cl["SELECT"])
+    tail = []
+    for c in ("WHERE", "GROUP", "HAVING", "ORDER", "LIMIT", "OFFSET"):
+        if c in cl and c != "HAVING":
+            tail += [c] + (["BY"] if c in ("GROUP", "ORDER") else []) + cl[c]
+    if "HAVING" not in cl:
+        names = _output_names(select)
+        steps.append(Step(" ".join(["SELECT"] + cl["SELECT"] + ["FROM"] + from_sql + tail) + ";", src, inner, names))
+        return len(steps) - 1
+    # HAVING: an Aggregate followed by a Filter is two compounds (RelAlgDagBuilder).  Step 1 computes the GROUP BY keys and
+    # every aggregate SELECT, HAVING or ORDER BY uses; step 2 projects the SELECT list out of it, filtered by the HAVING
+    # condition over its columns, then sorts and limits.
+    if "GROUP" not in cl:
+        raise ValueError("HAVING without GROUP BY")
+    keys = _split_commas(cl["GROUP"])
+    if any(len(k) != 1 for k in keys):
+        raise ValueError("GROUP BY expressions are outside this front-end")
+    key_names = [k[0].split(".")[-1].lower() for k in keys]
+    if len(set(key_names)) != len(key_names):
+        raise ValueError("two GROUP BY keys of one name")
+    aggs, agg_names = [], {}
+    out_names = _output_names(select)
+    for i, t in enumerate(select):
+        if _is_agg(t, 0):
+            text = _agg_text(t, 0)[0]
+            if text not in agg_names:
+                aggs.append(t[:t.index(")") + 1])
+                agg_names[text] = out_names[i] if out_names[i] not in key_names and not out_names[i].startswith("expr") \
+                    else f"agg{len(aggs) - 1}"
+        elif len(t) != 1 and not (len(t) == 3 and t[1].upper() == "AS") and len(t) != 2:
+            raise ValueError("expressions in the SELECT list are outside this front-end")
+    for c in ("HAVING", "ORDER"):
+        t = cl.get(c, [])
+        for j2 in range(len(t)):
+            if _is_agg(t, j2):
+                text, k = _agg_text(t, j2)
+                if text not in agg_names:
+                    aggs.append(t[j2:k])
+                    agg_names[text] = f"agg{len(aggs) - 1}"
+    step1 = ["SELECT", ", ".join(keys_[0] for keys_ in keys)] + [", " + " ".join(a) for a in aggs]
+    step1 = " ".join(step1).replace(" ,", ",")
+    tail1 = []
+    if "WHERE" in cl:
+        tail1 += ["WHERE"] + cl["WHERE"]
+    tail1 += ["GROUP", "BY"] + cl["GROUP"]
+    steps.append(Step(" ".join([step1, "FROM"] + from_sql + tail1) + ";", src, inner, key_names + list(agg_names.values())))
+    first = len(steps) - 1
+
+    def rewrite(t: List[str]) -> List[str]:
+        out, j2 = [], 0
+        while j2 < len(t):
+            if _is_agg(t, j2):
+                text, j2 = _agg_text(t, j2)
+                out.append(agg_names[text])
+                continue
+            tok = t[j2]
+            if re.fullmatch(r"[A-Za-z_][A-Za-z_0-9]*\.[A-Za-z_][A-Za-z_0-9]*", tok):
+                tok = tok.split(".")[-1]
+            out.append(tok)
+            j2 += 1
+        return out
+
+    proj = []
+    for i, t in enumerate(select):
+        col = agg_names[_agg_text(t, 0)[0]] if _is_agg(t, 0) else t[0].split(".")[-1].lower()
+        proj.append(col if col == out_names[i] or out_names[i].startswith("expr") else f"{col} AS {out_names[i]}")
+    tail2 = ["WHERE"] + rewrite(cl["HAVING"])
+    if "ORDER" in cl:
+        tail2 += ["ORDER", "BY"] + rewrite(cl["ORDER"])
+    for c in ("LIMIT", "OFFSET"):
+        if c in cl:
+            tail2 += [c] + cl[c]
+    names = [p.split(" AS ")[-1] for p in proj]
+    steps.append(Step(" ".join(["SELECT", ", ".join(proj), "FROM", f"tmp{first}"] + tail2) + ";", first, None, names))
+    return len(steps) - 1
+
+
+def parse_steps(sql: str, table: abi.Table, names: List[str], tables=None) -> List[Step]:
+    """The work units of `sql` in the order RelAlgDag makes them (an Aggregate followed by a Filter, a subquery in FROM
+    and an aggregated subquery on the inner side of a join each end a unit), for queries over temporary tables:
+
+        SELECT ... GROUP BY ... HAVING <cond> [ORDER BY ...] [LIMIT n] [OFFSET m]
+        SELECT ... FROM (SELECT ...) [alias] ...                       (nested to any depth)
+        SELECT ... FROM t [LEFT] JOIN (SELECT k, AGG(..) FROM d GROUP BY k) s ON t.a = s.k ...
+
+    Each step is a query parse() accepts, over a base table or the result of an earlier step (read as a temporary table
+    whose column names are that step's `names`).  `table` / `names` describe the table a FROM names when `tables`
+    ({name: (abi.Table, [column names])}) does not list it; parse() itself is unchanged.  Raises ValueError for a shape
+    outside this front-end."""
+    toks = _tokens(sql)
+    tables = {k.lower(): v for k, v in (tables or {}).items()}
+    for tok_i, tok in enumerate(toks):
+        up = tok.upper()
+        if up == "FROM" and toks[tok_i + 1] != "(" and toks[tok_i + 1].lower() not in tables:
+            tables[toks[tok_i + 1].lower()] = (table, list(names))
+    steps: List[Step] = []
+    _plan(toks, steps, tables)
+    return steps

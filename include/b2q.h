@@ -51,7 +51,8 @@ extern "C" {
                                B2Q_STAT_ROWS_SCANNED, TOTAL_MATCHED / MAX_MATCHED of b2q_launch;
                             8: B2Q_STAT_JOIN_TABLE (B2Q_JOIN_TABLE_*), b2q_last_launch_stat;
                             9: B2QExecutionOptions.with_dynamic_watchdog / dynamic_watchdog_time_limit /
-                               allow_runtime_query_interrupt / interrupt_token, b2q_interrupt_token_* / b2q_interrupt[_reset] */
+                               allow_runtime_query_interrupt / interrupt_token, b2q_interrupt_token_* / b2q_interrupt[_reset];
+                               additive, same version: b2q_device_columns_chunk_stats (temporary tables) */
 
 /* ---- SQLTypes subset (Shared/sqltypes.h:65-99) -------------------------------------------------------- */
 enum {
@@ -608,6 +609,22 @@ const void* b2q_device_columns_column(const B2QDeviceColumns* dc, size_t col, B2
                                       int64_t* null_count);
 int32_t b2q_device_columns_export_arrow(B2QDeviceColumns* dc, const char* const* names, struct ArrowSchema* schema,
                                         struct ArrowDeviceArray* array);
+/* synthesize_metadata (InputMetadata.cpp:381-470) of column `col`, computed by the conversion kernel in the same pass
+ * (no second read of the columns, no extra copy).  The stats are those of the encoder Encoder::Create(nullptr, type)
+ * picks (DataMgr/NoneEncoder.h): for integer-meta columns (integers, DECIMAL as scaled int64, TIME / TIMESTAMP / DATE,
+ * dictionary ids) a value is NULL iff it is the type's inline sentinel and int_min / int_max cover the others; FLOAT /
+ * DOUBLE columns treat FLT_MIN / DBL_MIN as NULL, never let a NaN into fp_min / fp_max, and give -0.0 and +0.0 either
+ * sign.  has_nulls = null_count > 0.  With no value in range (no rows, every value NULL or NaN): min =
+ * numeric_limits<T>::max() and max = numeric_limits<T>::lowest() of the column's type T.  The other pair is 0.
+ * NULL handle, NULL `out` or `col` out of range: B2Q_ERR_INVALID_ARGUMENT.
+ *
+ * A temporary table (the next step reading this result, ColumnFetcher::getResultSetColumn) is a B2QTableInfo of
+ *   - column types as b2q_device_columns_column reports them, DECIMAL scales included; col_encoded_sizes = NULL (no
+ *     encodings: a DATE column is 8-byte epoch seconds, dictionary ids are int32);
+ *   - memory_level B2Q_GPU_LEVEL and ONE fragment: fragment_id 0, device_id = b2q_device_columns_device, num_tuples =
+ *     b2q_device_columns_size, col_buffers = the column pointers, col_stats = these stats.
+ * It runs on that device only.  The caller keeps `dc` alive until the last call that reads the table has returned. */
+int32_t b2q_device_columns_chunk_stats(const B2QDeviceColumns* dc, size_t col, B2QChunkStats* out);
 void b2q_device_columns_free(B2QDeviceColumns* dc, void* cuda_stream);
 
 /* ---- synthetic data (bench / tests): counter-based generator, identical to oracle/oracle_gen.h ----------

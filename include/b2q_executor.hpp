@@ -296,6 +296,30 @@ class DeviceColumnarResults {
   size_t size() const { return b2q_device_columns_size(h_); }
   int deviceId() const { return b2q_device_columns_device(h_); }
   const SQLTypeInfo& getColumnType(const int col_id) const { return target_types_[col_id]; }
+  /* synthesize_metadata (InputMetadata.cpp:381-470) of one column, computed by the conversion (b2q_device_columns_chunk_stats) */
+  ChunkStats chunkStats(const int col_id) const {
+    B2QChunkStats s;
+    const int32_t rc = b2q_device_columns_chunk_stats(h_, static_cast<size_t>(col_id), &s);
+    if (rc != B2Q_OK) throw QueryExecutionError(rc, b2q_last_error_message());
+    return ChunkStats{s.int_min, s.int_max, s.fp_min, s.fp_max, s.has_nulls != 0};
+  }
+  /* the temporary table the next step reads (getResultSetColumn + synthesize_metadata): one GPU_LEVEL fragment, id 0, on
+   * deviceId(), over these columns and their stats.  This object must outlive every call that reads the table. */
+  InputTableInfo asTable() const {
+    InputTableInfo t;
+    t.col_types = target_types_;
+    t.memory_level = MemoryLevel::GPU_LEVEL;
+    FragmentInfo f;
+    f.fragmentId = 0;
+    f.deviceId = deviceId();
+    f.numTuples = size();
+    for (size_t c = 0; c < column_buffers_.size(); ++c) {
+      f.col_buffers.push_back(column_buffers_[c]);
+      f.chunkStats.push_back(chunkStats(static_cast<int>(c)));
+    }
+    t.fragments.push_back(std::move(f));
+    return t;
+  }
   /* Arrow C Device Data Interface record batch; the caller owns both structs and calls their release */
   void exportArrow(const std::vector<std::string>& names, ArrowSchema* schema, ArrowDeviceArray* array) const {
     std::vector<const char*> cn;

@@ -4,6 +4,7 @@ made tests/golden/executetest_harvest.json).  Harvest the reference's own golden
 committed as tests/golden/executetest_harvest.json and replayed by tests/test_oracle_golden_harvest.py without the reference).
 
     python tools/harvest_executetest.py <heavydb source tree> > tests/golden/executetest_harvest.json
+    python tools/harvest_executetest.py --steps <heavydb source tree> > tests/golden/executetest_steps_harvest.json
 
 Tests/ExecuteTest.cpp holds ~1350 `c("SELECT ...", dt)` comparisons against SQLite.  A string is kept when
   * it reads only table `test` and only the columns tests/ref_full_table.py models (the numeric, dictionary-string and FIXED columns
@@ -12,6 +13,9 @@ Tests/ExecuteTest.cpp holds ~1350 `c("SELECT ...", dt)` comparisons against SQLi
     GROUP BY columns, COUNT / SUM / MIN / MAX / AVG / COUNT(DISTINCT) of a column, ORDER BY / LIMIT / OFFSET),
   * the oracle plans it (the path's own refusals drop the rest), and
   * SQLite evaluates the same string.
+With --steps it keeps instead the strings of more than one work unit (HAVING, a subquery in FROM) that sqlmini.parse_steps splits
+and the oracle plans at EVERY step, each intermediate read as a host temporary table (tests/temp_table_ref.py); they are replayed by
+tests/test_temp_table_cpu.py and tests/test_gpu_temp_table.py.
 Only the query string and the reference line it came from are stored: the expected rows are recomputed with SQLite at test time,
 exactly as the reference's SQLiteComparator does (ExecuteTest.cpp:383-520)."""
 import json
@@ -27,10 +31,24 @@ import oracle_lib  # noqa: E402
 import ref_full_table as ft  # noqa: E402
 import ref_tables as rt  # noqa: E402
 import sqlmini  # noqa: E402
-from heavydb_b200 import abi  # noqa: E402
+from heavydb_b200 import abi, executor  # noqa: E402
+
+def accepts_steps(sql, table):
+    """parse_steps splits it into two or more steps and the oracle plans and runs every one of them."""
+    import temp_table_ref as tt
+    steps = sqlmini.parse_steps(sql, table, ft.FULL_NAMES)
+    if len(steps) < 2:
+        return False
+    tt.run_steps(steps, {"test": (table, ft.FULL_NAMES)},
+                 lambda i, unit, tbl, names: tt.run_step_on_host(steps[i], unit, tbl, names, 48),
+                 lambda _i, unit, tbl, res: tt.host_table(tt.oracle_columns(unit, tbl, res, 48)), dicts=ft.DICTS)
+    return True
+
 
 def main():
-    text = open(os.path.join(sys.argv[1], "Tests", "ExecuteTest.cpp")).read()
+    steps_mode = "--steps" in sys.argv[1:]
+    args = [a for a in sys.argv[1:] if a != "--steps"]
+    text = open(os.path.join(args[0], "Tests", "ExecuteTest.cpp")).read()
     rows = ft.full_rows()
     table = ft.make_table(rows)
     con = ft.make_sqlite(rows)
@@ -47,21 +65,38 @@ def main():
                 continue
             ln = text.count("\n", 0, m.start()) + 1
             stats["strings"] += 1
-            if not re.search(r"\bFROM test\b", q) or re.search(r"\b(JOIN|UNION|OVER|CASE|HAVING|EXTRACT|CAST|LIKE|DISTINCT ON)\b|,\s*test\b|\(SELECT", q, re.I):
+            if steps_mode:
+                if not re.search(r"\bFROM test\b", q) or not re.search(r"\bHAVING\b|\bFROM\s*\(\s*SELECT\b", q, re.I) or \
+                        re.search(r"\b(JOIN|UNION|OVER|CASE|EXTRACT|CAST|LIKE|DISTINCT ON)\b|,\s*test\b", q, re.I):
+                    continue
+            elif not re.search(r"\bFROM test\b", q) or re.search(r"\b(JOIN|UNION|OVER|CASE|HAVING|EXTRACT|CAST|LIKE|DISTINCT ON)\b|,\s*test\b|\(SELECT", q, re.I):
                 continue
             stats["table_test"] += 1
             sql = q if q.endswith(";") else q + ";"
             if sql in seen:
                 continue
-            try:
-                unit = sqlmini.parse(sql, table, ft.FULL_NAMES, dicts=ft.DICTS)
-            except Exception:
-                continue
-            stats["parsed"] += 1
-            try:
-                res = oracle_lib.execute(unit, table, entry_guess=48, has_card=True, num_threads=2)
-            except oracle_lib.OracleError:
-                continue
+            if steps_mode:
+                try:
+                    sqlmini.parse_steps(sql, table, ft.FULL_NAMES)
+                except Exception:
+                    continue
+                stats["parsed"] += 1
+                try:
+                    if not accepts_steps(sql, table):
+                        continue
+                except (oracle_lib.OracleError, executor.QueryExecutionError, ValueError, AssertionError, KeyError, IndexError):
+                    continue
+                res = None
+            else:
+                try:
+                    unit = sqlmini.parse(sql, table, ft.FULL_NAMES, dicts=ft.DICTS)
+                except Exception:
+                    continue
+                stats["parsed"] += 1
+                try:
+                    res = oracle_lib.execute(unit, table, entry_guess=48, has_card=True, num_threads=2)
+                except oracle_lib.OracleError:
+                    continue
             stats["planned"] += 1
             try:
                 con.execute(sql.rstrip(";")).fetchall()
@@ -71,7 +106,8 @@ def main():
             seen.add(sql)
             out.append({"sql": sql, "line": ln})
     stats["kept"] = len(out)
-    json.dump({"source": "Tests/ExecuteTest.cpp", "how": "tools/harvest_executetest.py", "stats": stats, "queries": out}, sys.stdout, indent=0)
+    how = "tools/harvest_executetest.py --steps" if steps_mode else "tools/harvest_executetest.py"
+    json.dump({"source": "Tests/ExecuteTest.cpp", "how": how, "stats": stats, "queries": out}, sys.stdout, indent=0)
     print()
     print(stats, file=sys.stderr)
 
